@@ -13,7 +13,7 @@ U64 = C.c_uint64
 DROP = [F, U32, U64]
 
 #: must equal dsvg_abi_version() of the loaded library (checked in _lib.load())
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 SIGNATURES = {
     "dsvg_abi_version": (I, []),
@@ -22,7 +22,6 @@ SIGNATURES = {
     "dsvg_outer_group": (I, [I, P, I, P]),
     "dsvg_linear_ln_fusable": (I, [I, I, I]),
     "dsvg_linear_ln_fwd": (I, [P, Z, I, P, Z, I, I, I, I, P, P, P, P, P, P, P]),
-    "dsvg_linear_ln_bwd": (I, [P, Z, I, P, Z, I, I, I, I, P, P, P, P, P, P, P] + DROP + [P, P, P]),
     "dsvg_pack_icons": (I, [P, P, I, I, I, I, P, P]),
     "dsvg_unpack_batch": (I, [P, P, P, P, Z, I, P]),
     "dsvg_match_assign": (I, [P, I, P, I, I, I, P, P, P, I, I, I, I, P, P, P, P, P, P]),

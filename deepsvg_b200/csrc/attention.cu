@@ -9,9 +9,8 @@
 // warp-broadcast float4s; the L x L probability tile never leaves shared memory.  Attention is 2.4 % of the step's
 // FLOPs (SURVEY.md 8d).  This file also holds the dispatcher of dsvg_attn_fwd / dsvg_attn_bwd: the tensor-core kernels of
 // attention_mma.cu take every shape of the BASELINE configs in both precision modes (one plane: attn_mma / attn_gmma,
-// two planes: attn_x3 / attn_gx3); the SIMT kernels below remain for head_dim 16, L > 80 and DSVG_ATTN=s (A/B switch).
+// two planes: attn_x3 / attn_gx3); the SIMT kernels below remain for head_dim 16 and L > 80.
 #include "../../include/dsvg_b200.h"
-#include <cstdlib>
 
 #include "common.cuh"
 
@@ -266,23 +265,19 @@ int dsvg_attn_x3(bool bwd, const bf16* qkv, size_t qkv_lo, const uint8_t* valid,
 int dsvg_attn_gx3(bool bwd, const bf16* qkv, size_t qkv_lo, const uint8_t* valid, bf16* out, size_t out_lo, const bf16* dout,
                   size_t dout_lo, bf16* dqkv, size_t dqkv_lo, int nseq, int L, int H, int head_dim, float q_scale, Dropout drop,
                   int causal, cudaStream_t st);
-static bool attn_simt_forced() {
-  static const bool off = [] { const char* e = getenv("DSVG_ATTN"); return e && e[0] == 's'; }();  // "simt"
-  return off;
-}
 static bool use_mma(bool single_plane, int L, int head_dim) {
-  return !attn_simt_forced() && single_plane && head_dim == 32 && L <= 32;
+  return single_plane && head_dim == 32 && L <= 32;
 }
 // parity mode (two planes everywhere) on the same 32 x 32 tiles: three bf16 products per contraction step
 static bool use_x3(bool two_planes, int L, int head_dim) {
-  return !attn_simt_forced() && two_planes && head_dim == 32 && L <= 32;
+  return two_planes && head_dim == 32 && L <= 32;
 }
 static bool use_gx3(bool two_planes, int L, int head_dim) {
-  return !attn_simt_forced() && two_planes && (head_dim == 32 || head_dim == 64) && L <= 80;
+  return two_planes && (head_dim == 32 || head_dim == 64) && L <= 80;
 }
 // general tensor-core kernel (attention_mma.cu): every other fast-mode shape of the BASELINE configs
 static bool use_gmma(bool single_plane, int L, int head_dim) {
-  return !attn_simt_forced() && single_plane && (head_dim == 32 || head_dim == 64) && L <= 80;
+  return single_plane && (head_dim == 32 || head_dim == 64) && L <= 80;
 }
 
 extern "C" int dsvg_attn_fwd(const dsvg_bf16* qkv, size_t qkv_lo_off, const uint8_t* key_valid, dsvg_bf16* out,

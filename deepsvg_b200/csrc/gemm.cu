@@ -13,7 +13,6 @@
 // Parity mode ("bf16x3"): operands carry a second bf16 plane (lo = v - bf16(v)); the consumers run three products
 // per K step (hi*hi + hi*lo + lo*hi) into the same accumulator.  Same kernel, NPLANES = 2.
 #include <cstdarg>
-#include <cstdlib>
 #include <cstring>
 #include <mutex>
 #include <unordered_map>
@@ -36,11 +35,6 @@ void set_error(const char* fmt, ...) {
 }
 const char* last_error() { return g_err; }
 unsigned long long g_launches = 0;
-bool pdl_enabled() {
-  static const bool on = [] { const char* e = getenv("DSVG_PDL"); return !(e && e[0] == '0'); }();
-  return on;
-}
-static uint32_t g_outer_lbo = 0, g_outer_sbo = 0;  // debug override of the MN-major descriptor strides
 
 // ------------------------------------------------------------------------------------------------
 // TMA tensor maps (host).  cuTensorMapEncodeTiled is fetched through the runtime so libcuda is not a link-time
@@ -145,21 +139,14 @@ struct Epi {
   size_t out_lo_off;
   int out_act_ld;
   int vec;   // 1: every pointer/stride satisfies the 4-wide vector path
-  int mode;  // 0: generic run-time epilogue; k > 0: lean epilogue kLeanFeat[k - 1]; 8 / 9: fused LayerNorm (see below)
-  // ---- fused LayerNorm (N == BN == 256: a CTA tile owns whole rows) ----
-  // mode 8 (forward):  x1 = residual epilogue of mode 4 -> out_f32;  ln_out = bf16(LN(x1) * gamma + beta); stats saved
-  // mode 9 (backward): dy = accumulator (dgrad into the LN output); dx_out = LN'(dy; x, mean, rstd, gamma) + dx_in;
-  //                    dact = bf16(dropout_mask * dx_out); dgamma / dbeta accumulated
+  int mode;  // 0: generic run-time epilogue; k > 0: lean epilogue kLeanFeat[k - 1]; 8: fused LayerNorm (see below)
+  // ---- mode 8, fused LayerNorm (N == BN == 256: a CTA tile owns whole rows) ----
+  // x1 = residual epilogue of mode 4 -> out_f32;  ln_out = bf16(LN(x1) * gamma + beta); mean / rstd saved
   const float* ln_gamma;
   const float* ln_beta;
-  bf16* ln_out;         // mode 8: [M, 256] ; mode 9: dact or null
-  float* ln_mean;       // mode 8: written ; mode 9: read
+  bf16* ln_out;         // [M, 256]
+  float* ln_mean;
   float* ln_rstd;
-  const float* ln_x;    // mode 9: the LayerNorm input (fp32 residual stream), row stride 256
-  const float* ln_dx_in;
-  float* ln_dx_out;
-  float* ln_dgamma;
-  float* ln_dbeta;
 };
 
 constexpr int kBlockM = 128;
@@ -284,32 +271,9 @@ __device__ __forceinline__ void epi_vec4(float4 x, long long row, int col, int N
 // this warp's private shared-memory tile so that every global access is a coalesced row segment.
 //   v[j]       : accumulator of row (row0 + lane), column (col0 + j)
 //   stage_addr : shared-space byte address of this warp's [32][36] fp32 staging tile
-template <bool kOuter>
 __device__ __forceinline__ void epilogue_chunk(uint32_t (&v)[32], uint32_t stage_addr, int lane, long long row0, int col0,
-                                               int M, int N, const Epi& ep, float alpha, float* C, int ldc) {
-  const float acc_scale = (!kOuter && ep.acc_scale_dev != nullptr) ? __ldg(ep.acc_scale_dev) : 1.f;
-  if constexpr (!kOuter) {
-    if (ep.vec == 2) {
-      // direct path: thread = row, eight aligned 4-column groups straight from the registers (no second smem round trip)
-      const long long row = row0 + lane;
-      if (row < M) {
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          const int col = col0 + 4 * q;
-          if (col < N) {
-            float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (ep.bias != nullptr) b4 = __ldg(reinterpret_cast<const float4*>(ep.bias + col));
-            EpiLoads l;
-            epi_vec4_load(l, row, col, ep);
-            epi_vec4(make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                                 __uint_as_float(v[4 * q + 3])),
-                     row, col, N, ep, b4, acc_scale, l);
-          }
-        }
-      }
-      return;
-    }
-  }
+                                               int M, int N, const Epi& ep) {
+  const float acc_scale = ep.acc_scale_dev != nullptr ? __ldg(ep.acc_scale_dev) : 1.f;
   {
     const uint32_t my = stage_addr + lane * (kStageRow * 4);
 #pragma unroll
@@ -318,15 +282,7 @@ __device__ __forceinline__ void epilogue_chunk(uint32_t (&v)[32], uint32_t stage
                    __uint_as_float(v[4 * q + 3]));
   }
   __syncwarp();
-  if constexpr (kOuter) {
-    const int col = col0 + lane;
-#pragma unroll 4
-    for (int r = 0; r < 32; ++r) {
-      long long row = row0 + r;
-      float x = ld_shared_f32(stage_addr + (r * kStageRow + lane) * 4);
-      if (row < M && col < N) atomicAdd(C + row * (long long)ldc + col, x * alpha);
-    }
-  } else if (ep.vec) {
+  if (ep.vec) {
     const int cg = lane & 7, rsub = lane >> 3;
     const int col = col0 + 4 * cg;
     const bool col_ok = col < N;
@@ -647,10 +603,10 @@ __host__ __device__ constexpr bool lin_tma_out(int mode, int nplanes = 1) {
 }
 // E consumer warps (E / 4 warpgroups issue the wgmma and then run the epilogue) + one TMA producer warp.
 __host__ __device__ constexpr int lin_epi_warps(int mode, int bn) {
-  // the fp32-residual epilogues (modes 4, 7, 8, 9) run 16 warps wide on the 256-wide tile: each thread then holds 64
+  // the fp32-residual epilogues (modes 4, 7, 8) run 16 warps wide on the 256-wide tile: each thread then holds 64
   // accumulator registers.  Mode 6 (head dgrads, K = 2827, light epilogue) and the TMA-store modes, whose bf16 output
   // tile takes 64 KB of shared memory, keep 8 warps so that two operand stages still fit.
-  return ((mode >= 3 && mode <= 9 && mode != 6 && !lin_tma_out(mode)) && bn == 256) ? 16 : 8;
+  return ((mode >= 3 && mode <= 8 && mode != 6 && !lin_tma_out(mode)) && bn == 256) ? 16 : 8;
 }
 
 
@@ -666,8 +622,9 @@ struct LinearCfg {
   // per-warp fragment transposition tiles; the staged epilogues use their staging tiles for it
   static constexpr int kXposeBytes = lin_tma_out(MODE, NPLANES) ? kEpiWarps * kStageWarpBytes : 0;
   static constexpr int kBiasBytes = BN * 4;   // bias slice of the current n-tile (TMA-out epilogues)
-  // fused LayerNorm: row partials [2 tile parities][128 rows][4 column quarters][2] + per-CTA dgamma / dbeta [2][256]
-  static constexpr int kLnBytes = (MODE == 8 || MODE == 9) ? (2 * 128 * 4 * 2 * 4 + 2 * 256 * 4) : 0;
+  // fused LayerNorm: row partials [2 tile parities][128 rows][4 column quarters][2], plus 2 KB that hold no data.  The
+  // 2 KB keep mode 8 at two operand stages, the configuration it is tuned and measured in; without them a third fits.
+  static constexpr int kLnBytes = MODE == 8 ? 2 * 128 * 4 * 2 * 4 + 2048 : 0;
   static constexpr int kFixedBytes = 1024 /*align slack*/ + kStagingBytes + kXposeBytes + 256 + kBiasBytes + kLnBytes;
   static constexpr int kMaxSmem = 227 * 1024;   // per-block dynamic shared memory limit of sm_90
   static constexpr int kStages = (kMaxSmem - kFixedBytes) / kStageBytes > 4 ? 4 : (kMaxSmem - kFixedBytes) / kStageBytes;
@@ -718,8 +675,7 @@ linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   uint64_t* empty_bar = bars + Cfg::kStages;       // [kStages]
   uint64_t* mfull_bar = bars + 2 * Cfg::kStages;   // [2] mask boxes of pass 0 / 1 have landed (mode 5)
   float* bias_sm = reinterpret_cast<float*>(xpose + Cfg::kXposeBytes + 256);
-  float* ln_part = bias_sm + BN;              // modes 8 / 9 only (Cfg::kLnBytes)
-  float* ln_acc = ln_part + 2 * 128 * 4 * 2;  // mode 9: [2][256] dgamma / dbeta of this CTA
+  float* ln_part = bias_sm + BN;              // mode 8 only (Cfg::kLnBytes)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -786,10 +742,6 @@ linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   } else {
     // =================== consumer warpgroups: wgmma main loop, then the epilogue ===================
     drop_resolve(ep.drop);
-    if constexpr (MODE == 9) {
-      for (int j = threadIdx.x; j < 512; j += Cfg::kEpiWarps * 32) ln_acc[j] = 0.f;
-      named_bar_sync(2, Cfg::kEpiWarps * 32);
-    }
     const int quarter = warp & 3;   // warp within its warpgroup: accumulator rows [32 quarter, 32 quarter + 32)
     const int half = warp >> 2;     // warpgroup: accumulator column chunks half * 32 + kCols * ci
     const uint32_t stage_buf = smem_u32(lin_tma_out(MODE, NPLANES) ? static_cast<void*>(xpose) : static_cast<void*>(staging)) +
@@ -857,7 +809,7 @@ linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
           if (n0 + c >= N) break;
           uint32_t v[32];
           acc_to_rows(accum[ci], stage_buf, lane, v);
-          epilogue_chunk<false>(v, stage_buf, lane, row0, n0 + c, M, N, ep, 1.f, nullptr, 0);
+          epilogue_chunk(v, stage_buf, lane, row0, n0 + c, M, N, ep);
         }
       } else if constexpr (MODE == 7) {
 #pragma unroll
@@ -1071,173 +1023,6 @@ linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
           }
         }
         continue;
-      } else if constexpr (MODE == 9) {
-        // ---------------- dgrad into a LayerNorm output + the LayerNorm backward of the finished rows ----------------
-        static_assert(BN == 256 && kCols == 128, "fused LayerNorm needs whole rows per CTA tile");
-        const int cg = lane & 7, rsub = lane >> 3;
-        float* part = ln_part + (it & 1) * (128 * 4 * 2);
-        float mean[8], rstd[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int row = int(row0) + rsub + 4 * i;
-          mean[i] = row < M ? __ldg(ep.ln_mean + row) : 0.f;
-          rstd[i] = row < M ? __ldg(ep.ln_rstd + row) : 0.f;
-        }
-        float4 g4[2];
-#pragma unroll
-        for (int ci = 0; ci < 2; ++ci)
-          g4[ci] = __ldg(reinterpret_cast<const float4*>(ep.ln_gamma + n0 + half * 32 + kCols * ci + 4 * cg));
-        float s1[8], s2[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) s1[i] = s2[i] = 0.f;
-        float4 xv[8];
-        {
-          const int col = n0 + half * 32 + 4 * cg;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int row = int(row0) + rsub + 4 * i;
-            if (row < M) xv[i] = *reinterpret_cast<const float4*>(ep.ln_x + size_t(row) * 256 + col);
-          }
-        }
-        // phase 1: row sums  s1 = sum_j dy_j g_j,  s2 = sum_j dy_j g_j xhat_j;  column sums for dgamma / dbeta
-#pragma unroll
-        for (int ci = 0; ci < 2; ++ci) {
-          const int c = half * 32 + kCols * ci;
-          uint32_t v[32];
-          acc_to_rows(accum[ci], stage_buf, lane, v);
-          {
-            const uint32_t my = stage_buf + lane * (kStageRow * 4);
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              st_shared_v4(my + q * 16, __uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                           __uint_as_float(v[4 * q + 3]));
-          }
-          __syncwarp();
-          const uint32_t lds_base = stage_buf + (rsub * kStageRow + 4 * cg) * 4;
-          float4 dgc = make_float4(0.f, 0.f, 0.f, 0.f), dbc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int row = int(row0) + rsub + 4 * i;
-            const float4 dy = ld_shared_v4(lds_base + i * (4 * kStageRow * 4));
-            if (row < M) {
-              const float4 xh = make_float4((xv[i].x - mean[i]) * rstd[i], (xv[i].y - mean[i]) * rstd[i],
-                                            (xv[i].z - mean[i]) * rstd[i], (xv[i].w - mean[i]) * rstd[i]);
-              const float4 t = make_float4(dy.x * g4[ci].x, dy.y * g4[ci].y, dy.z * g4[ci].z, dy.w * g4[ci].w);
-              s1[i] += (t.x + t.y) + (t.z + t.w);
-              s2[i] += (t.x * xh.x + t.y * xh.y) + (t.z * xh.z + t.w * xh.w);
-              dgc.x += dy.x * xh.x; dgc.y += dy.y * xh.y; dgc.z += dy.z * xh.z; dgc.w += dy.w * xh.w;
-              dbc.x += dy.x; dbc.y += dy.y; dbc.z += dy.z; dbc.w += dy.w;
-            }
-          }
-          __syncwarp();
-          // the 4 row groups of this warp share the lane's columns: fold them, then one shared-memory atomic per column
-          dgc.x += __shfl_xor_sync(0xffffffffu, dgc.x, 8); dgc.y += __shfl_xor_sync(0xffffffffu, dgc.y, 8);
-          dgc.z += __shfl_xor_sync(0xffffffffu, dgc.z, 8); dgc.w += __shfl_xor_sync(0xffffffffu, dgc.w, 8);
-          dbc.x += __shfl_xor_sync(0xffffffffu, dbc.x, 8); dbc.y += __shfl_xor_sync(0xffffffffu, dbc.y, 8);
-          dbc.z += __shfl_xor_sync(0xffffffffu, dbc.z, 8); dbc.w += __shfl_xor_sync(0xffffffffu, dbc.w, 8);
-          dgc.x += __shfl_xor_sync(0xffffffffu, dgc.x, 16); dgc.y += __shfl_xor_sync(0xffffffffu, dgc.y, 16);
-          dgc.z += __shfl_xor_sync(0xffffffffu, dgc.z, 16); dgc.w += __shfl_xor_sync(0xffffffffu, dgc.w, 16);
-          dbc.x += __shfl_xor_sync(0xffffffffu, dbc.x, 16); dbc.y += __shfl_xor_sync(0xffffffffu, dbc.y, 16);
-          dbc.z += __shfl_xor_sync(0xffffffffu, dbc.z, 16); dbc.w += __shfl_xor_sync(0xffffffffu, dbc.w, 16);
-          if (rsub == 0) {
-            float* ag = ln_acc + c + 4 * cg;
-            atomicAdd(ag + 0, dgc.x); atomicAdd(ag + 1, dgc.y); atomicAdd(ag + 2, dgc.z); atomicAdd(ag + 3, dgc.w);
-            atomicAdd(ag + 256, dbc.x); atomicAdd(ag + 257, dbc.y); atomicAdd(ag + 258, dbc.z); atomicAdd(ag + 259, dbc.w);
-          }
-          if (ci == 0) {
-            const int col = n0 + c + kCols + 4 * cg;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int row = int(row0) + rsub + 4 * i;
-              if (row < M) xv[i] = *reinterpret_cast<const float4*>(ep.ln_x + size_t(row) * 256 + col);
-            }
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          s1[i] = sum_cg(s1[i]);
-          s2[i] = sum_cg(s2[i]);
-        }
-        if (cg == 0) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            float2* dst = reinterpret_cast<float2*>(part + ((quarter * 32 + rsub + 4 * i) * 4 + half) * 2);
-            *dst = make_float2(s1[i], s2[i]);
-          }
-        }
-        named_bar_sync(3 + quarter, 128);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4* src = reinterpret_cast<const float4*>(part + (quarter * 32 + rsub + 4 * i) * 8);
-          const float4 p0 = src[0], p1 = src[1];
-          const float c1 = ((p0.x + p0.z) + (p1.x + p1.z)) * (1.f / 256.f);
-          const float c2 = ((p0.y + p0.w) + (p1.y + p1.w)) * (1.f / 256.f);
-          // dx = r (dy g - c1 - xhat c2) = dy (r g) + x B + C   with  B = -r^2 c2,  C = -r c1 + mean r^2 c2
-          const float r = rstd[i];
-          s2[i] = -r * r * c2;
-          s1[i] = -r * c1 - mean[i] * s2[i];
-        }
-        // phase 2: dx = rstd * (dy g - s1 - xhat s2) + dx_in  (second pass over the accumulator, x re-read from L2)
-        const bool has_drop = ep.drop.p > 0.f;
-#pragma unroll
-        for (int ci = 1; ci >= 0; --ci) {                 // xv still holds the columns of pass 1
-          const int c = half * 32 + kCols * ci;
-          const int col = n0 + c + 4 * cg;
-          if (ci == 0) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int row = int(row0) + rsub + 4 * i;
-              if (row < M) xv[i] = *reinterpret_cast<const float4*>(ep.ln_x + size_t(row) * 256 + col);
-            }
-          }
-          uint32_t v[32];
-          acc_to_rows(accum[ci], stage_buf, lane, v);
-          {
-            const uint32_t my = stage_buf + lane * (kStageRow * 4);
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              st_shared_v4(my + q * 16, __uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                           __uint_as_float(v[4 * q + 3]));
-          }
-          __syncwarp();
-          const uint32_t lds_base = stage_buf + (rsub * kStageRow + 4 * cg) * 4;
-          const unsigned long long quad0 =
-              ((unsigned long long)(int(row0) + rsub) * 256ull + (unsigned long long)col) >> 2;
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {                 // four rows at a time: their dx_in loads fly together
-            float4 din[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const int row = int(row0) + rsub + 4 * (4 * hh + k);
-              din[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (row < M && ep.ln_dx_in != nullptr) din[k] = *reinterpret_cast<const float4*>(ep.ln_dx_in + size_t(row) * 256 + col);
-            }
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int i = 4 * hh + k;
-            const int row = int(row0) + rsub + 4 * i;
-            const float4 dy = ld_shared_v4(lds_base + i * (4 * kStageRow * 4));
-            if (row < M) {
-              const float r = rstd[i];
-              float4 o;
-              o.x = dy.x * (r * g4[ci].x) + xv[i].x * s2[i] + s1[i] + din[k].x;
-              o.y = dy.y * (r * g4[ci].y) + xv[i].y * s2[i] + s1[i] + din[k].y;
-              o.z = dy.z * (r * g4[ci].z) + xv[i].z * s2[i] + s1[i] + din[k].z;
-              o.w = dy.w * (r * g4[ci].w) + xv[i].w * s2[i] + s1[i] + din[k].w;
-              if (ep.ln_dx_out != nullptr) *reinterpret_cast<float4*>(ep.ln_dx_out + size_t(row) * 256 + col) = o;
-              if (ep.ln_out != nullptr) {
-                if (has_drop) {
-                  const unsigned long long quad = quad0 + (unsigned long long)i * 256ull;   // row advances by 4: 4 * 256 / 4 quads
-                  const float4 mk = dropout_quad_mult(ep.drop, uint32_t(quad), drop_hikey(ep.drop, quad));
-                  o.x *= mk.x; o.y *= mk.y; o.z *= mk.z; o.w *= mk.w;
-                }
-                st_bf16x4(ep.ln_out + size_t(row) * 256 + col, o.x, o.y, o.z, o.w);
-              }
-            }
-          }
-          }
-          __syncwarp();
-        }
       } else {
         constexpr uint32_t FEAT = kLeanFeat[MODE > 0 ? MODE - 1 : 0];
         // residual / mask operands are fetched one chunk ahead: the first chunk's loads fly while the MMAs of this
@@ -1274,13 +1059,6 @@ linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     }
     if constexpr (lin_tma_out(MODE, NPLANES)) {
       if (warp == 0 && lane == 0) tma_store_wait_all();   // bulk stores must complete before the CTA's smem goes away
-    }
-    if constexpr (MODE == 9) {
-      named_bar_sync(2, Cfg::kEpiWarps * 32);             // every warp's shared-memory atomics have landed
-      for (int j = threadIdx.x; j < 512; j += Cfg::kEpiWarps * 32) {
-        float* dst = j < 256 ? ep.ln_dgamma : ep.ln_dbeta;
-        if (dst != nullptr) atomicAdd(dst + (j & 255), ln_acc[j]);
-      }
     }
   }
 }
@@ -1614,15 +1392,11 @@ static int launch_linear_split(const CUtensorMap& a, const CUtensorMap& alo, con
 
 // which lean epilogue (if any) covers exactly the requested steps
 static int pick_mode(const Epi& ep, bool split, int N) {
-  static const bool off = [] { const char* e = getenv("DSVG_EPI"); return e && e[0] == 'g'; }();  // "generic"
-  if (off) return 0;
   if (ep.vec == 0) {   // unaligned rows: only the plain "acc + bias -> fp32" head epilogue has a lean version
-    static const bool no7 = [] { const char* e = getenv("DSVG_EPI"); return e && e[0] == '7'; }();  // A/B switch
     const bool plain = ep.out_f32 && !ep.out_act && !ep.acc_scale_dev && ep.scale_cols == 0 && !ep.relu &&
                        !(ep.drop.p > 0.f) && !ep.rowvec && !ep.mask && !ep.residual;
-    return (plain && !no7) ? 7 : 0;
+    return plain ? 7 : 0;
   }
-  if (ep.vec != 1) return 0;
   if (!split && (ep.mask_lo_off != 0 || ep.out_lo_off != 0)) return 0;   // single-plane operands with two-plane outputs: generic
   uint32_t f = 0;
   if (ep.acc_scale_dev) f |= F_ACCS;
@@ -1678,8 +1452,7 @@ static int launch_outer(const CUtensorMap& a, const CUtensorMap& alo, const CUte
   splits = ceil_div(total_mblk, per);
   dim3 grid(out_tiles, splits);
   DSVG_CUDA(launch_k(outer_kernel<BQ, NPLANES>, grid, dim3(Cfg::kThreads), Cfg::kSmemBytes, st, a, alo, b, blo, M, P, Q, per, alpha,
-                     alpha_dev, C, ldc, colsum_out, g_outer_lbo ? g_outer_lbo : uint32_t(Cfg::kBoxBytes),
-                     g_outer_sbo ? g_outer_sbo : 1024u,
+                     alpha_dev, C, ldc, colsum_out, uint32_t(Cfg::kBoxBytes), 1024u,
                      int(ldc % 4 == 0 && Q % 4 == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0)));
   ++g_launches;
   return 0;
@@ -1690,11 +1463,7 @@ static int launch_outer(const CUtensorMap& a, const CUtensorMap& alo, const CUte
 using namespace dsvg;
 
 extern "C" const char* dsvg_last_error(void) { return dsvg::last_error(); }
-extern "C" int dsvg_abi_version(void) { return 5; }
-extern "C" void dsvg_debug_outer_desc(unsigned lbo, unsigned sbo) {
-  dsvg::g_outer_lbo = lbo;
-  dsvg::g_outer_sbo = sbo;
-}
+extern "C" int dsvg_abi_version(void) { return 6; }
 extern "C" unsigned long long dsvg_launch_count(void) { return dsvg::g_launches; }
 
 static int fill_epi(Epi& ep, const dsvg_epilogue* e, int M, int N) {
@@ -1728,8 +1497,7 @@ static int fill_epi(Epi& ep, const dsvg_epilogue* e, int M, int N) {
     v = v && (!ep.rowvec || ep.rowvec_ld % 4 == 0) && (!ep.residual || ep.res_ld % 4 == 0) &&
         (!ep.out_f32 || ep.out_f32_ld % 4 == 0) && (!ep.mask || (ep.mask_ld % 4 == 0 && ep.mask_lo_off % 4 == 0)) &&
         (!ep.out_act || (ep.out_act_ld % 4 == 0 && ep.out_lo_off % 4 == 0));
-    static const int direct = [] { const char* e = getenv("DSVG_EPI"); return (e && e[0] == 'd') ? 1 : 0; }();  // staged (transposed) epilogue measured 2.2x faster than direct
-    ep.vec = v ? (direct ? 2 : 1) : 0;
+    ep.vec = v ? 1 : 0;
   }
   return 0;
 }
@@ -1744,11 +1512,10 @@ extern "C" int dsvg_linear(const dsvg_bf16* X, size_t x_lo_off, int lda, const d
   if (fill_epi(ep, e, M, N)) return 1;
   DSVG_CHECK(ep.out_f32 || ep.out_act, "dsvg_linear: no output requested");
   const bool split = x_lo_off != 0;
-  static const bool force128 = [] { const char* e = getenv("DSVG_BN128"); return e && e[0] == '1'; }();
   // 256-wide tiles for the big path-level GEMMs; the group-level ones (M = N_icons * 8 rows, a few dozen tiles) run the
   // 128-wide kernel: twice the CTAs and two CTAs per SM shorten their latency-bound critical path.  Parity mode always
   // uses the 128-wide tile (shared-memory budget of the split planes).
-  const bool wide = (N > 128) && !split && !force128 && M > 16384;
+  const bool wide = (N > 128) && !split && M > 16384;
   const uint32_t bn = wide ? 256 : 128;
   CUtensorMap a, alo, b, blo;
   const bf16* Xb = reinterpret_cast<const bf16*>(X);
@@ -1771,25 +1538,17 @@ extern "C" int dsvg_linear(const dsvg_bf16* X, size_t x_lo_off, int lda, const d
 // GEMM + LayerNorm in one kernel (fast mode, d_model = 256 rows owned by one CTA tile, path-level row counts)
 // ---------------------------------------------------------------------------------------------------------------
 extern "C" int dsvg_linear_ln_fusable(int M, int N, int n_planes) {
-  static const bool off = [] { const char* e = getenv("DSVG_LN_FUSE"); return e && e[0] == '0'; }();
-  return (!off && n_planes == 1 && N == 256 && M > 16384) ? 1 : 0;
-}
-
-static int ln_common_checks(const dsvg_bf16* X, size_t x_lo_off, int lda, const dsvg_bf16* W, size_t w_lo_off, int ldb, int M,
-                            int N, int K) {
-  DSVG_CHECK(X && W, "dsvg_linear_ln: null pointer");
-  DSVG_CHECK(M > 0 && K > 0, "dsvg_linear_ln: bad shape");
-  DSVG_CHECK(lda % 8 == 0 && ldb % 8 == 0, "dsvg_linear_ln: lda/ldb must be multiples of 8 elements");
-  DSVG_CHECK(x_lo_off == 0 && w_lo_off == 0 && dsvg_linear_ln_fusable(M, N, 1),
-             "dsvg_linear_ln: shape / mode not fusable (ask dsvg_linear_ln_fusable first)");
-  return 0;
+  return (n_planes == 1 && N == 256 && M > 16384) ? 1 : 0;
 }
 
 extern "C" int dsvg_linear_ln_fwd(const dsvg_bf16* X, size_t x_lo_off, int lda, const dsvg_bf16* W, size_t w_lo_off, int ldb,
                                   int M, int N, int K, const dsvg_epilogue* e, const float* gamma, const float* beta,
                                   dsvg_bf16* y, float* mean, float* rstd, void* stream) {
-  if (ln_common_checks(X, x_lo_off, lda, W, w_lo_off, ldb, M, N, K)) return 1;
-  DSVG_CHECK(e && gamma && beta && y && mean && rstd, "dsvg_linear_ln_fwd: null pointer");
+  DSVG_CHECK(X && W && e && gamma && beta && y && mean && rstd, "dsvg_linear_ln_fwd: null pointer");
+  DSVG_CHECK(M > 0 && K > 0, "dsvg_linear_ln_fwd: bad shape");
+  DSVG_CHECK(lda % 8 == 0 && ldb % 8 == 0, "dsvg_linear_ln_fwd: lda/ldb must be multiples of 8 elements");
+  DSVG_CHECK(x_lo_off == 0 && w_lo_off == 0 && dsvg_linear_ln_fusable(M, N, 1),
+             "dsvg_linear_ln_fwd: shape / mode not fusable (ask dsvg_linear_ln_fusable first)");
   Epi ep{};
   if (fill_epi(ep, e, M, N)) return 1;
   DSVG_CHECK(ep.out_f32 && !ep.out_act && !ep.mask && !ep.relu && ep.scale_cols == 0 && !ep.acc_scale_dev && ep.vec == 1,
@@ -1802,29 +1561,6 @@ extern "C" int dsvg_linear_ln_fwd(const dsvg_bf16* X, size_t x_lo_off, int lda, 
   if (make_map(&a, reinterpret_cast<const bf16*>(X), K, M, lda, 64, 16)) return 1;
   if (make_map(&b, reinterpret_cast<const bf16*>(W), K, N, ldb, 64, 256)) return 1;
   return launch_linear_mode<256, 1, 8>(a, a, b, b, M, N, K, ep, static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int dsvg_linear_ln_bwd(const dsvg_bf16* dY, size_t dy_lo_off, int lda, const dsvg_bf16* W, size_t w_lo_off, int ldb,
-                                  int M, int N, int K, const float* x, const float* mean, const float* rstd,
-                                  const float* gamma, const float* dx_in, float* dx_out, dsvg_bf16* dact, float drop_p,
-                                  uint32_t drop_site, uint64_t seed, float* dgamma, float* dbeta, void* stream) {
-  if (ln_common_checks(dY, dy_lo_off, lda, W, w_lo_off, ldb, M, N, K)) return 1;
-  DSVG_CHECK(x && mean && rstd && gamma && (dx_out || dact), "dsvg_linear_ln_bwd: null pointer");
-  auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-  DSVG_CHECK(al16(x) && al16(gamma) && al16(dx_in) && al16(dx_out) && al16(dact),
-             "dsvg_linear_ln_bwd: x / gamma / dx_in / dx_out / dact must be 16-byte aligned");
-  Epi ep{};
-  ep.rows_per_group = 1;
-  ep.vec = 1;
-  ep.drop = make_dropout(drop_p, drop_site, seed);
-  ep.ln_x = x; ep.ln_mean = const_cast<float*>(mean); ep.ln_rstd = const_cast<float*>(rstd); ep.ln_gamma = gamma;
-  ep.ln_dx_in = dx_in; ep.ln_dx_out = dx_out; ep.ln_out = reinterpret_cast<bf16*>(dact);
-  ep.ln_dgamma = dgamma; ep.ln_dbeta = dbeta;
-  ep.mode = 9;
-  CUtensorMap a, b;
-  if (make_map(&a, reinterpret_cast<const bf16*>(dY), K, M, lda, 64, 16)) return 1;
-  if (make_map(&b, reinterpret_cast<const bf16*>(W), K, N, ldb, 64, 256)) return 1;
-  return launch_linear_mode<256, 1, 9>(a, a, b, b, M, N, K, ep, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int dsvg_outer_group(int n, const dsvg_outer_problem* pr, int M, void* stream) {
@@ -1863,8 +1599,7 @@ extern "C" int dsvg_outer_group(int n, const dsvg_outer_problem* pr, int M, void
     DSVG_CUDA(cudaFuncSetAttribute(outer_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   }
   DSVG_CUDA(launch_k(outer_group_kernel, dim3(g.cta_begin[n]), dim3(Cfg::kThreads), Cfg::kSmemBytes,
-                     static_cast<cudaStream_t>(stream), g, g_outer_lbo ? g_outer_lbo : uint32_t(Cfg::kBoxBytes),
-                     g_outer_sbo ? g_outer_sbo : 1024u));
+                     static_cast<cudaStream_t>(stream), g, uint32_t(Cfg::kBoxBytes), 1024u));
   ++g_launches;
   return 0;
 }

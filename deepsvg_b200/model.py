@@ -36,23 +36,6 @@ def _r8(n):
     return (n + 7) // 8 * 8
 
 
-class _Range:
-    """NVTX range around a phase of the step (DSVG_NVTX=1): `ncu --nvtx --nvtx-include "dsvg/E1.fwd/"` profiles one stack."""
-    on = os.environ.get("DSVG_NVTX", "0") == "1"
-
-    def __init__(self, name):
-        self.name = name
-
-    def __enter__(self):
-        if _Range.on:
-            torch.cuda.nvtx.range_push("dsvg/" + self.name)
-
-    def __exit__(self, *a):
-        if _Range.on:
-            torch.cuda.nvtx.range_pop()
-        return False
-
-
 # ======================================================================================================
 # parameter inventory (names / shapes / initialisers of the reference module tree, SURVEY.md 8b)
 # ======================================================================================================
@@ -283,7 +266,6 @@ class SVGTransformer(nn.Module):
         self._sites = {}
         self._wcache = {}
         self._eps_override = None      # tests inject the VAE noise here (SURVEY.md 8c hazard 2)
-        self.wgrad_group = os.environ.get("DSVG_WGRAD_GROUP", "1") != "0"   # one weight-gradient launch per block
 
     # -------------------------------------------------------------------------------------------------
     def _param(self, name):
@@ -616,16 +598,14 @@ class SVGTransformer(nn.Module):
         nxt = None
         for i in range(n_layers):
             lp = "%s.layers.%d" % (pre, i)
-            with _Range(lp + ".fwd.globals"):
-                rv = self._globals_fwd(sv, lp, zmem, nseq, lab, lab_rpg) if (zmem is not None or lab is not None) else None
+            rv = self._globals_fwd(sv, lp, zmem, nseq, lab, lab_rpg) if (zmem is not None or lab is not None) else None
             rpg = L if zmem is not None else lab_rows_per_group
             if i + 1 < n_layers:
                 nl = "%s.layers.%d" % (pre, i + 1)
                 next_ln = (self._param(nl + ".norm1.weight"), self._param(nl + ".norm1.bias"))
             else:
                 next_ln = (self._param(pre + ".norm.weight"), self._param(pre + ".norm.bias")) if final_ln else None
-            with _Range(lp + ".fwd"):
-                x, nxt = self._layer_fwd(sv, lp, x, M, L, nseq, key_valid, rv, rpg, a_pre=nxt, next_ln=next_ln)
+            x, nxt = self._layer_fwd(sv, lp, x, M, L, nseq, key_valid, rv, rpg, a_pre=nxt, next_ln=next_ln)
         return x, nxt
 
     def _forward_impl(self, inp, seed_dev=None):
@@ -918,7 +898,7 @@ class SVGTransformer(nn.Module):
         # (12.0 vs 12.2 ms): those stay separate launches.
         t256 = lambda n: (n + 255) // 256
         n_tiles = t256(3 * d) * t256(d) + t256(d) * t256(d) + 2 * t256(ff) * t256(d)
-        grouped = [] if (pl == 1 and M >= 16384 and self.wgrad_group and n_tiles <= 16) else None
+        grouped = [] if (pl == 1 and M >= 16384 and n_tiles <= 16) else None
 
         def wgrad(A, B, P_, Q_, w, b):
             if grouped is None:
@@ -931,20 +911,13 @@ class SVGTransformer(nn.Module):
         _, w2t = self._pack(pre + ".linear2.weight")
         ops.linear(dx2_act, w2t, M, ff, d, mask=s["h"], mask_scale=1.0 / (1.0 - pff[0]) if pff[0] > 0 else 1.0, out_act=dh)
         wgrad(dh, s["b"], ff, d, G("linear1.weight"), G("linear1.bias"))
-        # The fused dgrad + LayerNorm-backward kernel (dsvg_linear_ln_bwd) is correct (tests/test_kernels_gpu.py) but its
-        # two-pass epilogue runs register-capped at 17 warps per SM and spills, so it is opt-in: DSVG_LN_FUSE_BWD=1.
-        fuse = ops.ln_fusable(M, d, pl) and os.environ.get("DSVG_LN_FUSE_BWD", "0") == "1"
         _, w1t = self._pack(pre + ".linear1.weight")
         dx1 = torch.empty(M, d, device=dev)
         dt = Act(M, d, pl, dev)
-        if fuse:    # FFN1 input gradient + LayerNorm-2 backward in one kernel: the bf16 gradient `db` never exists in HBM
-            ops.linear_ln_bwd(dh, w1t, M, d, ff, s["x1"], s["mean2"], s["rstd2"], P("norm2.weight"), dx_in=dx2, dx_out=dx1,
-                              dact=dt, drop=self._drop(sv, pre + ".drop1"), dgamma=G("norm2.weight"), dbeta=G("norm2.bias"))
-        else:
-            db = Act(M, d, pl, dev)
-            ops.linear(dh, w1t, M, d, ff, out_act=db)
-            ops.ln_bwd(s["x1"], s["mean2"], s["rstd2"], P("norm2.weight"), M, d, dy=db, dx_in=dx2, dx_out=dx1, dact=dt,
-                       drop=self._drop(sv, pre + ".drop1"), dgamma=G("norm2.weight"), dbeta=G("norm2.bias"))
+        db = Act(M, d, pl, dev)
+        ops.linear(dh, w1t, M, d, ff, out_act=db)
+        ops.ln_bwd(s["x1"], s["mean2"], s["rstd2"], P("norm2.weight"), M, d, dy=db, dx_in=dx2, dx_out=dx1, dact=dt,
+                   drop=self._drop(sv, pre + ".drop1"), dgamma=G("norm2.weight"), dbeta=G("norm2.bias"))
         # ---- attention ----
         wgrad(dt, s["o"], d, d, G("self_attn.out_proj.weight"), G("self_attn.out_proj.bias"))
         do = Act(M, d, pl, dev)
@@ -957,14 +930,10 @@ class SVGTransformer(nn.Module):
         _, wit = self._pack(pre + ".self_attn.in_proj_weight")
         dx0 = torch.empty(M, d, device=dev)
         dx0_act = Act(M, d, pl, dev) if want_dact else None
-        if fuse:
-            ops.linear_ln_bwd(dqkv, wit, M, d, 3 * d, s["x"], s["mean1"], s["rstd1"], P("norm1.weight"), dx_in=dx1,
-                              dx_out=dx0, dact=dx0_act, drop=prev_drop, dgamma=G("norm1.weight"), dbeta=G("norm1.bias"))
-        else:
-            da = Act(M, d, pl, dev)
-            ops.linear(dqkv, wit, M, d, 3 * d, out_act=da)
-            ops.ln_bwd(s["x"], s["mean1"], s["rstd1"], P("norm1.weight"), M, d, dy=da, dx_in=dx1, dx_out=dx0, dact=dx0_act,
-                       drop=prev_drop, dgamma=G("norm1.weight"), dbeta=G("norm1.bias"))
+        da = Act(M, d, pl, dev)
+        ops.linear(dqkv, wit, M, d, 3 * d, out_act=da)
+        ops.ln_bwd(s["x"], s["mean1"], s["rstd1"], P("norm1.weight"), M, d, dy=da, dx_in=dx1, dx_out=dx0, dact=dx0_act,
+                   drop=prev_drop, dgamma=G("norm1.weight"), dbeta=G("norm1.bias"))
         if grouped:
             ops.outer_group(grouped, M)
         return dx0, dx0_act, dx1
@@ -1008,8 +977,7 @@ class SVGTransformer(nn.Module):
         for i in reversed(range(n_layers)):
             lp = "%s.layers.%d" % (pre, i)
             prev = self._drop(sv, "%s.layers.%d.drop2" % (pre, i - 1)) if i > 0 else (0.0, 0, 0)
-            with _Range(lp + ".bwd"):
-                dx, dx_act, dx1 = self._layer_bwd(sv, gd, lp, dx, dx_act, M, L, nseq, key_valid, prev, want_dact=i > 0)
+            dx, dx_act, dx1 = self._layer_bwd(sv, gd, lp, dx, dx_act, M, L, nseq, key_valid, prev, want_dact=i > 0)
             if zmem is not None or lab is not None:
                 self._globals_bwd(sv, gd, lp, dx1, nseq, L, zmem, dzmem, lab, dlab, lab_rows_per_group, lab_rpg)
         return dx

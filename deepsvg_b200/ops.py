@@ -78,7 +78,7 @@ def act_from_float(x, planes, ld=None):
 
 
 def ln_fusable(M, N, planes):
-    """True when the GEMM's CTA tile owns whole LayerNorm rows, so that linear_ln_fwd / linear_ln_bwd apply."""
+    """True when the GEMM's CTA tile owns whole LayerNorm rows, so that the fused LayerNorm of linear(ln=...) applies."""
     return bool(_lib.load().dsvg_linear_ln_fusable(M, N, planes))
 
 
@@ -117,18 +117,6 @@ def linear(X, W, M, N, K, *, bias=None, scale_cols=0, scale=1.0, relu=False, dro
     with _Prof("linear", 2.0 * M * N * K, (M, N, K), nb):
         rc = _lib.load().dsvg_linear(X.ptr, X.lo, X.ld, W.ptr, W.lo, W.ld, M, N, K, C.byref(ep), _stream())
     _lib.check(rc, "dsvg_linear")
-
-
-def linear_ln_bwd(dY, W, M, N, K, x, mean, rstd, gamma, *, dx_in=None, dx_out=None, dact=None, drop=(0.0, 0, 0),
-                  dgamma=None, dbeta=None):
-    """dgrad GEMM dY[M,K] . W[N,K]^T whose result is the gradient at a LayerNorm output, fused with that LayerNorm's
-    backward (see include/dsvg_b200.h); same outputs as linear(..., out_act=dy) followed by ln_bwd(dy=dy, ...)."""
-    with _Prof("linear", 2.0 * M * N * K, (M, N, K)):
-        rc = _lib.load().dsvg_linear_ln_bwd(dY.ptr, dY.lo, dY.ld, W.ptr, W.lo, W.ld, M, N, K, x.data_ptr(), mean.data_ptr(),
-                                            rstd.data_ptr(), gamma.data_ptr(), _p(dx_in), _p(dx_out),
-                                            dact.ptr if dact is not None else 0, drop[0], drop[1], drop[2], _p(dgamma),
-                                            _p(dbeta), _stream())
-    _lib.check(rc, "dsvg_linear_ln_bwd")
 
 
 def outer(A, B, M, P, Q, Cout, *, alpha=1.0, alpha_dev=None, colsum=None):

@@ -103,24 +103,15 @@ int dsvg_outer_group(int n_problems, const dsvg_outer_problem* problems, int M, 
 
 /* GEMM + LayerNorm in one kernel (fast mode).  When the CTA tile of dsvg_linear owns whole rows (N = d_model = 256,
  * path-level row counts, single-plane operands: ask dsvg_linear_ln_fusable) the LayerNorm that follows a residual-stream
- * linear, and the LayerNorm backward that follows the input-gradient GEMM of the layer's QKV / FFN1 linear, run in that
- * GEMM's epilogue: the fp32 residual stream is not re-read by a separate kernel and the bf16 dgrad never goes to HBM.
- *   forward  (improved_transformer.py:43-44 -> :51, :52-53 -> next layer's :43 / transformer.py:185-186):
+ * linear runs in that GEMM's epilogue: the fp32 residual stream is not re-read by a separate kernel.
+ *   (improved_transformer.py:43-44 -> :51, :52-53 -> next layer's :43 / transformer.py:185-186):
  *       x1 = epilogue `e` (bias, dropout, row vector, residual -> e->out_f32 [M,256], row stride e->out_f32_ld)
  *       y  = bf16(LayerNorm(x1) * gamma + beta) [M,256];  mean[M], rstd[M] saved for the backward
- *   backward (autograd of the same lines):  dy = dY[M,K] . W[256,K]^T  (stays on chip)
- *       dx_out = rstd * (dy*gamma - mean_j(dy*gamma) - xhat * mean_j(dy*gamma*xhat)) + dx_in      (fp32 [M,256])
- *       dact   = bf16(dropout_mask(drop_p, site, seed)[row*256+col] * dx_out)                      (optional)
- *       dgamma += sum_rows dy * xhat ;  dbeta += sum_rows dy                                        (optional)
- * Results equal dsvg_linear followed by dsvg_ln_fwd / dsvg_ln_bwd (tests/test_kernels_gpu.py). */
+ * Results equal dsvg_linear followed by dsvg_ln_fwd (tests/test_kernels_gpu.py). */
 int dsvg_linear_ln_fusable(int M, int N, int n_planes);
 int dsvg_linear_ln_fwd(const dsvg_bf16* X, size_t x_lo_off, int lda, const dsvg_bf16* W, size_t w_lo_off, int ldb, int M,
                        int N, int K, const dsvg_epilogue* e, const float* gamma, const float* beta, dsvg_bf16* y,
                        float* mean, float* rstd, void* stream);
-int dsvg_linear_ln_bwd(const dsvg_bf16* dY, size_t dy_lo_off, int lda, const dsvg_bf16* W, size_t w_lo_off, int ldb, int M,
-                       int N, int K, const float* x, const float* mean, const float* rstd, const float* gamma,
-                       const float* dx_in, float* dx_out, dsvg_bf16* dact, float drop_p, uint32_t drop_site, uint64_t seed,
-                       float* dgamma, float* dbeta, void* stream);
 
 /* ---- input side: packed batch format (SURVEY.md 8f rank 3) --------------------------------------------- */
 /* HOST function.  Assembles one batch the way SVGTensorDataset.get_data does per icon (svgtensor_dataset.py:164-205 with

@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol():
     assert len(fns) >= 28
     for name in fns:
         assert hasattr(lib, name), name
-    assert lib.dsvg_abi_version() == 5
+    assert lib.dsvg_abi_version() == 6
     assert lib.dsvg_launch_count() == 0          # nothing launched: loading needs no GPU
 
 

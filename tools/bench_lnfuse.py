@@ -1,6 +1,5 @@
-"""Development microbenchmark: fused GEMM+LayerNorm kernels against their two-kernel equivalents at the path-level shape
-(M = 131072 rows, d_model = 256), CUDA-event timed.  `python tools/bench_lnfuse.py [which]` (which: all | fwd | bwd | one of
-the ncu targets lnfwd / lnbwd512 / lnbwd768, which only launch the fused kernel a few times)."""
+"""Development microbenchmark: the fused GEMM+LayerNorm forward kernel against its two-kernel equivalent at the path-level
+shape (M = 131072 rows, d_model = 256), CUDA-event timed.  `python tools/bench_lnfuse.py`"""
 import os
 import sys
 
@@ -9,7 +8,6 @@ import torch
 from deepsvg_b200 import ops
 
 dev = torch.device("cuda:0")
-which = sys.argv[1] if len(sys.argv) > 1 else "all"
 M, N = 131072, 256
 
 
@@ -40,53 +38,17 @@ bias = torch.zeros(N, device=dev)
 x1 = [torch.empty(M, N, device=dev) for _ in range(2)]
 y = [ops.Act(M, N, 1, dev) for _ in range(2)]
 
-if which in ("all", "fwd", "lnfwd"):
-    for K in (256, 512):
-        X, W = act(M, K), act(N, K, K ** -0.5)
-        i = [0]
+for K in (256, 512):
+    X, W = act(M, K), act(N, K, K ** -0.5)
+    i = [0]
 
-        def fused():
-            j = i[0] = i[0] ^ 1
-            ops.linear(X, W, M, N, K, bias=bias, drop=(0.1, 4, 7), residual=res, out_f32=x1[j], ln=(g, b, y[j], mean, rstd))
+    def fused():
+        j = i[0] = i[0] ^ 1
+        ops.linear(X, W, M, N, K, bias=bias, drop=(0.1, 4, 7), residual=res, out_f32=x1[j], ln=(g, b, y[j], mean, rstd))
 
-        def split():
-            j = i[0] = i[0] ^ 1
-            ops.linear(X, W, M, N, K, bias=bias, drop=(0.1, 4, 7), residual=res, out_f32=x1[j])
-            ops.ln_fwd(x1[j], g, b, y[j], mean, rstd, M, N)
+    def split():
+        j = i[0] = i[0] ^ 1
+        ops.linear(X, W, M, N, K, bias=bias, drop=(0.1, 4, 7), residual=res, out_f32=x1[j])
+        ops.ln_fwd(x1[j], g, b, y[j], mean, rstd, M, N)
 
-        if which == "lnfwd":
-            for _ in range(4):
-                fused()
-            torch.cuda.synchronize()
-        else:
-            print("fwd  K=%d  fused %.1f us   linear+ln_fwd %.1f us" % (K, timeit(fused), timeit(split)), flush=True)
-
-if which in ("all", "bwd", "lnbwd512", "lnbwd768"):
-    x = torch.randn(M, N, device=dev)
-    dxin = torch.randn(M, N, device=dev)
-    dx = [torch.empty(M, N, device=dev) for _ in range(2)]
-    dg, db = torch.zeros(N, device=dev), torch.zeros(N, device=dev)
-    dyb = ops.Act(M, N, 1, dev)
-    for K in (512, 768):
-        if which.startswith("lnbwd") and which != "lnbwd%d" % K:
-            continue
-        dY, Wt = act(M, K), act(N, K, K ** -0.5)
-        i = [0]
-
-        def fused():
-            j = i[0] = i[0] ^ 1
-            ops.linear_ln_bwd(dY, Wt, M, N, K, x, mean, rstd, g, dx_in=dxin, dx_out=dx[j], dact=y[j], drop=(0.1, 4, 7),
-                              dgamma=dg, dbeta=db)
-
-        def split():
-            j = i[0] = i[0] ^ 1
-            ops.linear(dY, Wt, M, N, K, out_act=dyb)
-            ops.ln_bwd(x, mean, rstd, g, M, N, dy=dyb, dx_in=dxin, dx_out=dx[j], dact=y[j], drop=(0.1, 4, 7), dgamma=dg,
-                       dbeta=db)
-
-        if which.startswith("lnbwd"):
-            for _ in range(4):
-                fused()
-            torch.cuda.synchronize()
-        else:
-            print("bwd  K=%d  fused %.1f us   dgrad+ln_bwd %.1f us" % (K, timeit(fused), timeit(split)), flush=True)
+    print("fwd  K=%d  fused %.1f us   linear+ln_fwd %.1f us" % (K, timeit(fused), timeit(split)), flush=True)

@@ -1,4 +1,4 @@
-"""Development helper for ncu: warm-up steps + profiled train steps of a bench workload (eager launches, no CUDA graph).
+"""Development helper for torch.profiler: train steps of a bench workload with eager launches (no CUDA graph).
 usage: python tools/one_step.py [batch] [steps] [config]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-"""Development tool: launch one hot linear shape / epilogue mode a few times (for `ncu -k regex:linear_kernel`)."""
+"""Development tool: launch one hot linear shape / epilogue mode a few times (to time it under torch.profiler)."""
 import os
 import sys
 
