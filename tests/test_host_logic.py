@@ -65,6 +65,27 @@ def test_unsupported_variants_raise_at_construction(over):
         SVGTransformer(Hierarchical(**over))
 
 
+def test_attention_length_limit_matches_the_shared_memory_formula():
+    """The longest sequence per head_dim is the largest L whose SIMT-backward tiles (Q, K, V, dO: L x hd; P, dS: L x (L | 1),
+    fp32) fit the 227 KB opt-in shared memory; one more position raises at construction, and the message quotes the
+    limits in tokens (two positions fewer: SOS and EOS)."""
+    import re
+    from deepsvg_b200 import OneStageOneShot, SVGTransformer
+    from deepsvg_b200.config import check_supported
+    from tests.test_kernels_gpu import ATTN_MAX_L
+
+    def fits(L, hd):
+        return 4 * (4 * L * hd + 2 * L * (L | 1) + 3) <= 227 * 1024
+
+    for hd, L in ATTN_MAX_L.items():
+        assert fits(L, hd) and not fits(L + 1, hd), hd
+        check_supported(OneStageOneShot(d_model=128, n_heads=128 // hd, max_total_len=L - 2))
+        with pytest.raises(NotImplementedError) as e:
+            SVGTransformer(OneStageOneShot(d_model=128, n_heads=128 // hd, max_total_len=L - 1))
+        quoted = re.search(r"limits: (\d+) / (\d+) / (\d+) tokens for head_dim 16 / 32 / 64", str(e.value))
+        assert quoted and [int(t) for t in quoted.groups()] == [ATTN_MAX_L[h] - 2 for h in (16, 32, 64)], str(e.value)
+
+
 def test_self_matching_variant_is_constructible_and_has_no_path_positional_code():
     """model/config.py:101-108, model.py:114-115."""
     from deepsvg_b200 import HierarchicalSelfMatching, OneStageOneShot, SVGTransformer

@@ -59,6 +59,9 @@ CASES = {
     "one_stage_fonts": ("one_stage", dict(use_vae=True, label_condition=True, n_labels=52, max_total_len=50), 5),
     "small_d128": ("hierarchical", dict(use_vae=False, d_model=128, n_heads=4, dim_feedforward=256, dim_z=64, n_layers=2,
                                         n_layers_decode=2, max_num_groups=4, max_seq_len=10), 6),
+    # attention on the fp32 SIMT kernels end to end: head_dim 16, and a one-stage sequence of 102 positions (> 80)
+    "hier_hd16": ("hierarchical", dict(use_vae=False, d_model=128, n_heads=8), 2),
+    "one_stage_long": ("one_stage", dict(use_vae=False, d_model=256, n_heads=4, max_total_len=100), 2),
 }
 
 
