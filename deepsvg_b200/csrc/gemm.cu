@@ -454,20 +454,6 @@ __device__ __forceinline__ void epilogue_chunk_lean(uint32_t (&v)[32], uint32_t 
   __syncwarp();
 }
 
-// sum over the 8 lanes that share a row group (lane bits 0..2 = column group)
-__device__ __forceinline__ float sum_cg(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  v += __shfl_xor_sync(0xffffffffu, v, 2);
-  v += __shfl_xor_sync(0xffffffffu, v, 4);
-  return v;
-}
-__device__ __forceinline__ void st_bf16x4(bf16* p, float a, float b, float c, float d) {
-  __nv_bfloat162 h0 = __floats2bfloat162_rn(a, b), h1 = __floats2bfloat162_rn(c, d);
-  uint2 u;
-  u.x = *reinterpret_cast<uint32_t*>(&h0);
-  u.y = *reinterpret_cast<uint32_t*>(&h1);
-  *reinterpret_cast<uint2*>(p) = u;
-}
 
 // feature sets with a compiled lean epilogue (index = Epi::mode - 1)
 constexpr uint32_t kLeanFeat[] = {
@@ -603,17 +589,37 @@ __host__ __device__ constexpr bool lin_tma_out(int mode, int nplanes = 1) {
 }
 // E consumer warps (E / 4 warpgroups issue the wgmma and then run the epilogue) + one TMA producer warp.
 __host__ __device__ constexpr int lin_epi_warps(int mode, int bn) {
-  // the fp32-residual epilogues (modes 4, 7, 8) run 16 warps wide on the 256-wide tile: each thread then holds 64
-  // accumulator registers.  Mode 6 (head dgrads, K = 2827, light epilogue) and the TMA-store modes, whose bf16 output
-  // tile takes 64 KB of shared memory, keep 8 warps so that two operand stages still fit.
-  return ((mode >= 3 && mode <= 8 && mode != 6 && !lin_tma_out(mode)) && bn == 256) ? 16 : 8;
+  // mode 7 (fp32 rows of any alignment) runs 16 warps wide on the 256-wide tile: each thread then holds 64 accumulator
+  // registers.  Mode 6 (head dgrads, K = 2827, light epilogue) keeps 8 warps.
+  return (mode == 7 && bn == 256) ? 16 : 8;
+}
+// The 256-wide single-plane kernels of the path-level GEMM roles (modes 1-5 and the fused LayerNorm 8) run the
+// full-width kernel below (linear_wide): two consumer warpgroups with one m64n256 wgmma per k16 step each, and the
+// epilogue applied to the accumulator fragments.
+__host__ __device__ constexpr bool lin_wide(int mode, int bn, int nplanes) {
+  return bn == 256 && nplanes == 1 && ((mode >= 1 && mode <= 5) || mode == 8);
 }
 
+template <int MODE>
+struct WideCfg {
+  static constexpr int kThreads = 384;                   // consumer warpgroups 0 and 1, producer warpgroup 2
+  static constexpr int kStages = 4;
+  static constexpr int kABytes = kBlockM * kBlockK * 2;  // 16 KB: warpgroup g reads rows [64 g, 64 g + 64)
+  static constexpr int kBBytes = 256 * kBlockK * 2;      // 32 KB, read by both warpgroups
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  static constexpr int kBoxBytes = 64 * 128;             // one [64 rows][64 bf16 columns] output box, 128-byte swizzle
+  // bf16 outputs (mode 8: the LayerNorm output) leave through a two-box ring per consumer warpgroup
+  static constexpr int kStagingBytes = MODE == 4 ? 0 : 2 * 2 * kBoxBytes;
+  static constexpr int kSmemBytes = 1024 /*align slack*/ + kStages * kStageBytes + kStagingBytes + 256 /*barriers*/;
+  static_assert(kSmemBytes <= 227 * 1024, "linear_wide: shared memory over the per-block limit of sm_90");
+};
 
 template <int BN, int NPLANES, int MODE = 0>
 struct LinearCfg {
+  static constexpr bool kWide = lin_wide(MODE, BN, NPLANES);
   static constexpr int kEpiWarps = lin_epi_warps(MODE, BN);
-  static constexpr int kThreads = 32 * kEpiWarps + 32;    // the producer is the last warp (consumers stay warpgroup-aligned)
+  // staged kernel: the producer is the last warp (consumers stay warpgroup-aligned)
+  static constexpr int kThreads = kWide ? WideCfg<MODE>::kThreads : 32 * kEpiWarps + 32;
   static constexpr int kChunks = BN / (8 * kEpiWarps);    // 32-column accumulator chunks per consumer warp
   static constexpr int kABytes = kBlockM * kBlockK * 2;  // 16 KB
   static constexpr int kBBytes = BN * kBlockK * 2;       // 16/32 KB
@@ -622,14 +628,11 @@ struct LinearCfg {
   // per-warp fragment transposition tiles; the staged epilogues use their staging tiles for it
   static constexpr int kXposeBytes = lin_tma_out(MODE, NPLANES) ? kEpiWarps * kStageWarpBytes : 0;
   static constexpr int kBiasBytes = BN * 4;   // bias slice of the current n-tile (TMA-out epilogues)
-  // fused LayerNorm: row partials [2 tile parities][128 rows][4 column quarters][2], plus 2 KB that hold no data.  The
-  // 2 KB keep mode 8 at two operand stages, the configuration it is tuned and measured in; without them a third fits.
-  static constexpr int kLnBytes = MODE == 8 ? 2 * 128 * 4 * 2 * 4 + 2048 : 0;
-  static constexpr int kFixedBytes = 1024 /*align slack*/ + kStagingBytes + kXposeBytes + 256 + kBiasBytes + kLnBytes;
+  static constexpr int kFixedBytes = 1024 /*align slack*/ + kStagingBytes + kXposeBytes + 256 + kBiasBytes;
   static constexpr int kMaxSmem = 227 * 1024;   // per-block dynamic shared memory limit of sm_90
   static constexpr int kStages = (kMaxSmem - kFixedBytes) / kStageBytes > 4 ? 4 : (kMaxSmem - kFixedBytes) / kStageBytes;
   static_assert(kStages >= 2, "linear: at least two pipeline stages must fit");
-  static constexpr int kSmemBytes = kFixedBytes + kStages * kStageBytes;
+  static constexpr int kSmemBytes = kWide ? WideCfg<MODE>::kSmemBytes : kFixedBytes + kStages * kStageBytes;
 };
 
 // One 32 x 32 chunk of a consumer warp's accumulators, a[h] = fragment of the m64 half h (local rows [16 h, 16 h + 16)),
@@ -657,12 +660,13 @@ __device__ __forceinline__ void acc_to_rows(const float (&a)[2][16], uint32_t st
   __syncwarp();
 }
 
+// Staged kernel (every linear_kernel instantiation but the full-width ones): consumer warps issue n32 wgmmas and
+// drain the accumulators 32 x 32 chunks at a time through per-warp transposition tiles.  The tensor maps are the
+// kernel's __grid_constant__ parameters.
 template <int BN, int NPLANES, int MODE>
-__global__ void __launch_bounds__((LinearCfg<BN, NPLANES, MODE>::kThreads), 1)
-linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmAlo,
-              const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBlo,
-              const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmM, int M, int N, int K,
-              Epi ep) {
+__device__ __forceinline__ void linear_staged(const CUtensorMap& tmA, const CUtensorMap& tmAlo, const CUtensorMap& tmB,
+                                              const CUtensorMap& tmBlo, const CUtensorMap& tmC, const CUtensorMap& tmM,
+                                              int M, int N, int K, Epi ep) {
   using Cfg = LinearCfg<BN, NPLANES, MODE>;
   constexpr int kCols = Cfg::kEpiWarps * 8;   // accumulator columns drained per pass of all epilogue warps (64 or 128)
   extern __shared__ uint8_t smem_raw[];
@@ -675,7 +679,6 @@ linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   uint64_t* empty_bar = bars + Cfg::kStages;       // [kStages]
   uint64_t* mfull_bar = bars + 2 * Cfg::kStages;   // [2] mask boxes of pass 0 / 1 have landed (mode 5)
   float* bias_sm = reinterpret_cast<float*>(xpose + Cfg::kXposeBytes + 256);
-  float* ln_part = bias_sm + BN;              // mode 8 only (Cfg::kLnBytes)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -905,124 +908,6 @@ linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
           }
         }
         continue;
-      } else if constexpr (MODE == 8) {
-        // ---------------- residual epilogue (as mode 4) + LayerNorm of the finished rows ----------------
-        static_assert(BN == 256 && kCols == 128, "fused LayerNorm needs whole rows per CTA tile");
-        const int cg = lane & 7, rsub = lane >> 3;
-        const int r_first = int(row0) + rsub;
-        float* part = ln_part + (it & 1) * (128 * 4 * 2);
-        const bool has_rv = ep.rowvec != nullptr, has_drop = ep.drop.p > 0.f, has_res = ep.residual != nullptr;
-        float rs[8], rq[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) rs[i] = rq[i] = 0.f;
-#pragma unroll
-        for (int ci = 0; ci < 2; ++ci) {
-          const int c = half * 32 + kCols * ci;
-          const int col = n0 + c + 4 * cg;
-          const float4 bias4 = ep.bias != nullptr ? __ldg(reinterpret_cast<const float4*>(ep.bias + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
-          uint32_t v[32];
-          acc_to_rows(accum[ci], stage_buf, lane, v);
-          {
-            const uint32_t my = stage_buf + lane * (kStageRow * 4);
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              st_shared_v4(my + q * 16, __uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                           __uint_as_float(v[4 * q + 3]));
-          }
-          __syncwarp();
-          const uint32_t lds_base = stage_buf + (rsub * kStageRow + 4 * cg) * 4;
-          const unsigned long long quad0 = ((unsigned long long)r_first * 256ull + (unsigned long long)col) >> 2;
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {                  // four rows at a time: their residual loads fly together
-            float4 res[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const int row = r_first + 4 * (4 * hh + k);
-              res[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (row < M && has_res) res[k] = *reinterpret_cast<const float4*>(ep.residual + size_t(row) * ep.res_ld + col);
-            }
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const int i = 4 * hh + k;
-              const int row = r_first + 4 * i;
-              float4 x = ld_shared_v4(lds_base + i * (4 * kStageRow * 4));
-              if (row < M) {
-                x.x += bias4.x; x.y += bias4.y; x.z += bias4.z; x.w += bias4.w;
-                if (has_drop) {
-                  const unsigned long long quad = quad0 + (unsigned long long)i * 256ull;   // row advances by 4
-                  const float4 m = dropout_quad_mult(ep.drop, uint32_t(quad), drop_hikey(ep.drop, quad));
-                  x.x *= m.x; x.y *= m.y; x.z *= m.z; x.w *= m.w;
-                }
-                if (has_rv) {
-                  const uint32_t grp = ep.rpg_magic ? __umulhi(uint32_t(row), ep.rpg_magic) : uint32_t(row / ep.rows_per_group);
-                  const float4 rv = __ldg(reinterpret_cast<const float4*>(ep.rowvec + size_t(grp) * ep.rowvec_ld + col));
-                  x.x += rv.x; x.y += rv.y; x.z += rv.z; x.w += rv.w;
-                }
-                x.x += res[k].x; x.y += res[k].y; x.z += res[k].z; x.w += res[k].w;
-                *reinterpret_cast<float4*>(ep.out_f32 + size_t(row) * ep.out_f32_ld + col) = x;
-                rs[i] += (x.x + x.y) + (x.z + x.w);
-                rq[i] += (x.x * x.x + x.y * x.y) + (x.z * x.z + x.w * x.w);
-              }
-            }
-          }
-          __syncwarp();
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          rs[i] = sum_cg(rs[i]);
-          rq[i] = sum_cg(rq[i]);
-        }
-        if (cg == 0) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            float2* dst = reinterpret_cast<float2*>(part + ((quarter * 32 + rsub + 4 * i) * 4 + half) * 2);
-            *dst = make_float2(rs[i], rq[i]);
-          }
-        }
-        named_bar_sync(3 + quarter, 128);                 // the four warps that share these 32 rows
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {                     // rs <- mean, rq <- rstd
-          const float4* src = reinterpret_cast<const float4*>(part + (quarter * 32 + rsub + 4 * i) * 8);
-          const float4 p0 = src[0], p1 = src[1];          // (s, q) of column quarters 0, 1 | 2, 3
-          const float sm = (p0.x + p0.z) + (p1.x + p1.z), sq = (p0.y + p0.w) + (p1.y + p1.w);
-          rs[i] = sm * (1.f / 256.f);
-          rq[i] = rsqrtf(fmaxf(sq * (1.f / 256.f) - rs[i] * rs[i], 0.f) + 1e-5f);
-        }
-        if (half == 0 && cg == 0) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int row = r_first + 4 * i;
-            if (row < M) {
-              ep.ln_mean[row] = rs[i];
-              ep.ln_rstd[row] = rq[i];
-            }
-          }
-        }
-#pragma unroll
-        for (int ci = 0; ci < 2; ++ci) {
-          const int col = n0 + half * 32 + kCols * ci + 4 * cg;
-          const float4 g4 = __ldg(reinterpret_cast<const float4*>(ep.ln_gamma + col));
-          const float4 b4 = __ldg(reinterpret_cast<const float4*>(ep.ln_beta + col));
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            float4 xv[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {                 // this lane's own stores of phase 1 (L2 hits)
-              const int row = r_first + 4 * (4 * hh + k);
-              if (row < M) xv[k] = *reinterpret_cast<const float4*>(ep.out_f32 + size_t(row) * ep.out_f32_ld + col);
-            }
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const int i = 4 * hh + k;
-              const int row = r_first + 4 * i;
-              const float sc = rq[i], sh = -rs[i] * rq[i];   // (x - mean) rstd = x sc + sh
-              if (row < M)
-                st_bf16x4(ep.ln_out + size_t(row) * 256 + col, (xv[k].x * sc + sh) * g4.x + b4.x, (xv[k].y * sc + sh) * g4.y + b4.y,
-                          (xv[k].z * sc + sh) * g4.z + b4.z, (xv[k].w * sc + sh) * g4.w + b4.w);
-            }
-          }
-        }
-        continue;
       } else {
         constexpr uint32_t FEAT = kLeanFeat[MODE > 0 ? MODE - 1 : 0];
         // residual / mask operands are fetched one chunk ahead: the first chunk's loads fly while the MMAs of this
@@ -1061,6 +946,294 @@ linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       if (warp == 0 && lane == 0) tma_store_wait_all();   // bulk stores must complete before the CTA's smem goes away
     }
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Full-width kernel (lin_wide): persistent over 128 x 256 CTA tiles in the staged kernel's round-robin order.
+// Warpgroup 2 produces: one elected lane streams the A [128 x 64] and B [256 x 64] k-blocks of each tile through four
+// stages, so B is loaded once per 128 output rows.  Consumer warpgroup g accumulates rows [64 g, 64 g + 64) of the tile
+// with one m64n256k16 wgmma per k16 step and runs the epilogue on the accumulator fragments, in which thread (w, lane)
+// of the warpgroup holds
+//   acc[4 j + 2 i + e] = D[16 w + lane / 4 + 8 i][8 j + 2 (lane % 4) + e]
+// i.e. column pairs of two rows; the four lanes of a quad cover 8 contiguous columns of a row.  bf16 outputs go through
+// a swizzled two-box ring and leave by TMA store; fp32 outputs and the residual / mask operands are accessed in the
+// fragment layout directly.
+// ------------------------------------------------------------------------------------------------
+template <uint32_t FEAT>
+struct WidePre {   // global operands of one 64-column box, [i][jj] = rows (i), column pairs 8 jj + 2 (lane % 4)
+  float2 res[(FEAT & F_RES) ? 16 : 1];
+  uint32_t mk[(FEAT & F_MASK) ? 16 : 1];
+};
+template <uint32_t FEAT>
+__device__ __forceinline__ void wide_prefetch(WidePre<FEAT>& p, int row0, int col0, int M, int N, const Epi& ep) {
+  if constexpr ((FEAT & (F_RES | F_MASK)) != 0) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        const int row = row0 + 8 * i, col = col0 + 8 * jj;
+        const bool ok = row < M && col < N;
+        if constexpr (FEAT & F_RES)
+          p.res[8 * i + jj] = (ok && ep.residual != nullptr)
+                                  ? *reinterpret_cast<const float2*>(ep.residual + size_t(row) * ep.res_ld + col)
+                                  : make_float2(0.f, 0.f);
+        if constexpr (FEAT & F_MASK)
+          p.mk[8 * i + jj] = ok ? *reinterpret_cast<const uint32_t*>(ep.mask + size_t(row) * ep.mask_ld + col) : 0u;
+      }
+  }
+}
+__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
+  __nv_bfloat162 t = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&t);
+}
+// One [64 x 64] bf16 box of a consumer warpgroup's tile -> ring buffer -> TMA store at (c0, r0).  word(i, jj) is this
+// thread's column pair jj of row i.  The warpgroup's leader thread issues the stores, so it alone tracks their groups.
+template <class Word>
+__device__ __forceinline__ void wide_box_out(uint8_t* ring, int& nbox, int bar_id, bool leader, int w, int lane,
+                                             const CUtensorMap* tm, int c0, int r0, Word word) {
+  if (leader) tma_store_wait_read_n<1>();   // the box stored from this buffer two boxes ago has been read out
+  named_bar_sync(bar_id, 128);
+  uint8_t* box = ring + (nbox & 1) * WideCfg<0>::kBoxBytes;
+  const int rq = lane >> 2;                 // == row & 7: the row's 16-byte chunk swizzle
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    uint8_t* rowp = box + (16 * w + 8 * i + rq) * 128 + 4 * (lane & 3);
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) *reinterpret_cast<uint32_t*>(rowp + ((jj ^ rq) << 4)) = word(i, jj);
+  }
+  fence_proxy_async_smem();                 // generic-proxy smem writes -> visible to the TMA engine
+  named_bar_sync(bar_id, 128);
+  if (leader) {
+    tma_store_2d(tm, box, c0, r0);
+    tma_store_commit();
+  }
+  ++nbox;
+}
+
+template <int MODE>
+__device__ __forceinline__ void linear_wide(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, int M,
+                                            int N, int K, Epi ep) {
+  using Cfg = WideCfg<MODE>;
+  // mode 8 is the residual epilogue of mode 4 followed by the LayerNorm of the finished rows (N == 256)
+  constexpr uint32_t FEAT = kLeanFeat[(MODE == 8 ? 4 : MODE) - 1];
+  constexpr bool kBoxOut = (FEAT & F_OUTA) != 0 || MODE == 8;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* tiles = smem;
+  uint8_t* rings = smem + Cfg::kStages * Cfg::kStageBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(rings + Cfg::kStagingBytes);
+  uint64_t* empty_bar = full_bar + Cfg::kStages;
+
+  const int wg = threadIdx.x >> 7;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x == 256) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int s = 0; s < Cfg::kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);   // one arrival per consumer warp
+    }
+    fence_barrier_init();
+  }
+  pdl_launch_dependents();
+  __syncthreads();
+  pdl_wait();   // everything above touched only this CTA's shared memory
+
+  const int n_tiles = (N + 255) / 256;
+  const int num_tiles = ((M + kBlockM - 1) / kBlockM) * n_tiles;
+  const int num_kb = (K + kBlockK - 1) / kBlockK;
+
+  if (wg == 2) {
+    // =================== producer warpgroup: registers go to the consumers, one warp issues ===================
+    setmaxnreg_dec<40>();
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles && warp == 8; tile += gridDim.x) {
+      const int m0 = (tile / n_tiles) * kBlockM;
+      const int n0 = (tile % n_tiles) * 256;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        if (elect_one()) {
+          uint8_t* st = tiles + stage * Cfg::kStageBytes;
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+#pragma unroll
+          for (int r = 0; r < kBlockM; r += 16) tma_load_2d(st + r * 128, &tmA, &full_bar[stage], kb * kBlockK, m0 + r);
+          tma_load_2d(st + Cfg::kABytes, &tmB, &full_bar[stage], kb * kBlockK, n0);
+        }
+        __syncwarp();
+        if (++stage == Cfg::kStages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+    }
+  } else {
+  // =================== consumer warpgroups ===================
+  // 40 (producer) x 128 + 232 x 256 = 64512 registers = 168 (the launch-bounds count) x 384
+  setmaxnreg_inc<232>();
+  drop_resolve(ep.drop);
+  const int w = warp & 3, q = lane & 3;
+  const int rloc = 16 * w + (lane >> 2);    // warpgroup-local row of acc[4 j + e]; acc[4 j + 2 + e] is 8 rows further
+  const bool leader = (threadIdx.x & 127) == 0;
+  uint8_t* ring = rings + wg * 2 * Cfg::kBoxBytes;
+  const bool has_bias = (FEAT & F_BIAS) && ep.bias != nullptr;
+  const bool has_drop = (FEAT & F_DROP) && ep.drop.p > 0.f;
+  const bool has_rv = (FEAT & F_ROWVEC) && ep.rowvec != nullptr;
+  int stage = 0;
+  uint32_t phase = 0;
+  int nbox = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int m0 = (tile / n_tiles) * kBlockM;
+    const int n0 = (tile % n_tiles) * 256;
+    const int row0 = m0 + 64 * wg + rloc;
+    float acc[128];
+#pragma unroll
+    for (int j = 0; j < 128; ++j) acc[j] = 0.f;
+    int prev_stage = 0;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      wgmma_fence();
+      const uint32_t a = smem_u32(tiles + stage * Cfg::kStageBytes) + wg * 8192;
+      const uint32_t b = smem_u32(tiles + stage * Cfg::kStageBytes) + Cfg::kABytes;
+#pragma unroll
+      for (int k = 0; k < kBlockK / 16; ++k)
+        wgmma_m64n256_kk(acc, gmma_smem_desc(a + k * 32, 16, 1024), gmma_smem_desc(b + k * 32, 16, 1024));
+      wgmma_commit();
+      if (kb > 0) {
+        wgmma_wait<1>();                                    // the previous k-block's MMAs have read their stage
+        if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      }
+      prev_stage = stage;
+      if (++stage == Cfg::kStages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    // the first box's residual / mask loads fly while the last MMAs finish.  The fp32 residual boxes (32 registers
+    // each) are single-buffered, refilled right after their last use, to stay within the register budget.
+    constexpr int kPre = (FEAT & F_RES) ? 1 : 2;
+    WidePre<FEAT> pre[kPre];
+    wide_prefetch<FEAT>(pre[0], row0, n0 + 2 * q, M, N, ep);
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+    if (m0 + 64 * wg < M) {                 // warpgroup-uniform: otherwise all of its rows are past the matrix
+
+      unsigned long long rowq[2];               // dropout quad index of (row, 0); N % 4 == 0 on every lean mode
+      uint32_t grp[2];
+      float s[2] = {0.f, 0.f}, ss[2] = {0.f, 0.f};   // mode 8: row sums of x1 and x1^2 (this thread's columns)
+  #pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int row = row0 + 8 * i;
+        rowq[i] = (unsigned long long)row * (unsigned long long)(N >> 2);
+        grp[i] = (has_rv && row < M) ? (ep.rpg_magic ? __umulhi(uint32_t(row), ep.rpg_magic) : uint32_t(row / ep.rows_per_group)) : 0u;
+      }
+  #pragma unroll
+      for (int bx = 0; bx < 4; ++bx) {
+        const int c0 = n0 + 64 * bx;            // first column of the box
+        if (c0 >= N) break;                     // CTA-uniform
+        if (kPre == 2 && bx < 3) wide_prefetch<FEAT>(pre[(bx + 1) & 1], row0, c0 + 64 + 2 * q, M, N, ep);
+        const WidePre<FEAT>& p = pre[bx & (kPre - 1)];
+  #pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int col = c0 + 8 * jj + 2 * q;  // even; col < N covers col + 1 as N % 4 == 0
+          float2 bias = make_float2(0.f, 0.f);
+          if (has_bias && col < N) bias = __ldg(reinterpret_cast<const float2*>(ep.bias + col));
+  #pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            float& x0 = acc[4 * (8 * bx + jj) + 2 * i];
+            float& x1 = acc[4 * (8 * bx + jj) + 2 * i + 1];
+            const int row = row0 + 8 * i;
+            if constexpr (FEAT & F_BIAS) { x0 += bias.x; x1 += bias.y; }
+            if constexpr (FEAT & F_SCALE) {
+              if (col < ep.scale_cols) { x0 *= ep.scale; x1 *= ep.scale; }
+            }
+            if constexpr (FEAT & F_RELU) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+            if constexpr (FEAT & F_DROP) {
+              if (has_drop) {   // this pair is half (lane % 2) of quad (row N + col) / 4, as dropout_quad_mult draws it
+                const unsigned long long quad = rowq[i] + uint32_t(col >> 2);
+                const uint32_t s1 = drop_stage1(uint32_t(quad), drop_hikey(ep.drop, quad));
+                const uint32_t h = (q & 1) ? drop_fin_b(s1) : drop_fin_a(s1);
+                x0 = drop_keep_lo(h, ep.drop.thr16) ? x0 * ep.drop.scale : 0.f;
+                x1 = drop_keep_hi(h, ep.drop.thr16) ? x1 * ep.drop.scale : 0.f;
+              }
+            }
+            if constexpr (FEAT & F_ROWVEC) {
+              if (has_rv && row < M && col < N) {
+                const float2 rv = __ldg(reinterpret_cast<const float2*>(ep.rowvec + size_t(grp[i]) * ep.rowvec_ld + col));
+                x0 += rv.x; x1 += rv.y;
+              }
+            }
+            if constexpr (FEAT & F_MASK) {   // a bf16 is non-zero iff any of its 15 magnitude bits is set
+              const uint32_t m = p.mk[8 * i + jj];
+              x0 = (m & 0x7FFFu) ? x0 * ep.mask_scale : 0.f;
+              x1 = (m & 0x7FFF0000u) ? x1 * ep.mask_scale : 0.f;
+            }
+            if constexpr (FEAT & F_RES) { x0 += p.res[8 * i + jj].x; x1 += p.res[8 * i + jj].y; }
+            if constexpr (FEAT & F_OUTF) {
+              if (row < M && col < N) *reinterpret_cast<float2*>(ep.out_f32 + size_t(row) * ep.out_f32_ld + col) = make_float2(x0, x1);
+            }
+            if constexpr (MODE == 8) {
+              s[i] += x0 + x1;
+              ss[i] += x0 * x0 + x1 * x1;
+            }
+          }
+        }
+        if (kPre == 1 && bx < 3) wide_prefetch<FEAT>(pre[0], row0, c0 + 64 + 2 * q, M, N, ep);
+        if constexpr ((FEAT & F_OUTA) != 0) {
+          wide_box_out(ring, nbox, 1 + wg, leader, w, lane, &tmC, c0, m0 + 64 * wg, [&](int i, int jj) {
+            return pack_bf16x2(acc[4 * (8 * bx + jj) + 2 * i], acc[4 * (8 * bx + jj) + 2 * i + 1]);
+          });
+        }
+      }
+      if constexpr (MODE == 8) {
+        // a quad holds whole rows: its four lanes' partial sums make the row's
+        float sc[2], sh[2];
+  #pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          s[i] += __shfl_xor_sync(0xffffffffu, s[i], 1);
+          s[i] += __shfl_xor_sync(0xffffffffu, s[i], 2);
+          ss[i] += __shfl_xor_sync(0xffffffffu, ss[i], 1);
+          ss[i] += __shfl_xor_sync(0xffffffffu, ss[i], 2);
+          const float mean = s[i] * (1.f / 256.f);
+          const float rstd = rsqrtf(fmaxf(ss[i] * (1.f / 256.f) - mean * mean, 0.f) + 1e-5f);
+          sc[i] = rstd;                          // (x - mean) rstd = x sc + sh
+          sh[i] = -mean * rstd;
+          const int row = row0 + 8 * i;
+          if (q == 0 && row < M) {
+            ep.ln_mean[row] = mean;
+            ep.ln_rstd[row] = rstd;
+          }
+        }
+  #pragma unroll
+        for (int bx = 0; bx < 4; ++bx) {
+          wide_box_out(ring, nbox, 1 + wg, leader, w, lane, &tmC, 64 * bx, m0 + 64 * wg, [&](int i, int jj) {
+            const int col = 64 * bx + 8 * jj + 2 * q;
+            const float2 g = __ldg(reinterpret_cast<const float2*>(ep.ln_gamma + col));
+            const float2 be = __ldg(reinterpret_cast<const float2*>(ep.ln_beta + col));
+            const float x0 = acc[4 * (8 * bx + jj) + 2 * i], x1 = acc[4 * (8 * bx + jj) + 2 * i + 1];
+            return pack_bf16x2((x0 * sc[i] + sh[i]) * g.x + be.x, (x1 * sc[i] + sh[i]) * g.y + be.y);
+          });
+        }
+      }
+    }
+    // bulk stores must complete before the CTA's smem goes away.  Waited for inside the tile loop: after the loop, the
+    // wait costs the consumer warpgroups their setmaxnreg budget (ptxas then allocates 168 registers).
+    if (kBoxOut && w == 0 && tile + int(gridDim.x) >= num_tiles) tma_store_wait_all();
+  }
+  }
+}
+
+template <int BN, int NPLANES, int MODE>
+__global__ void __launch_bounds__((LinearCfg<BN, NPLANES, MODE>::kThreads), 1)
+linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmAlo,
+              const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBlo,
+              const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmM, int M, int N, int K,
+              Epi ep) {
+  if constexpr (lin_wide(MODE, BN, NPLANES))
+    linear_wide<MODE>(tmA, tmB, tmC, M, N, K, ep);
+  else
+    linear_staged<BN, NPLANES, MODE>(tmA, tmAlo, tmB, tmBlo, tmC, tmM, M, N, K, ep);
 }
 
 // 16-byte vector reduction (REDG.E.ADD.F32x4): four consecutive fp32 gradient entries per instruction
@@ -1342,7 +1515,13 @@ template <int BN, int NPLANES, int MODE>
 static int launch_linear_mode(const CUtensorMap& a, const CUtensorMap& alo, const CUtensorMap& b, const CUtensorMap& blo,
                               int M, int N, int K, const Epi& ep, cudaStream_t st) {
   CUtensorMap c = a, mk = a;
-  if (lin_tma_out(MODE, NPLANES)) {
+  if (lin_wide(MODE, BN, NPLANES)) {   // 64 x 64 output boxes, one consumer warpgroup's rows each
+    if (MODE == 8) {
+      if (make_map(&c, ep.ln_out, 256, M, 256, 64, 64)) return 1;
+    } else if (lin_tma_out(MODE, NPLANES)) {
+      if (make_map(&c, ep.out_act, N, M, ep.out_act_ld, 64, 64)) return 1;
+    }
+  } else if (lin_tma_out(MODE, NPLANES)) {
     if (make_map(&c, ep.out_act, N, M, ep.out_act_ld, 64, 128)) return 1;
     if (ep.mask != nullptr && make_map(&mk, ep.mask, N, M, ep.mask_ld, 64, 128)) return 1;
   }
