@@ -37,6 +37,9 @@ SIGNATURES = {
     "dsvg_ln_bwd": (I, [P, P, P, P, P, Z, P, P, P, I, P, P, P, Z] + DROP + [P, P, I, I, P]),
     "dsvg_attn_fwd": (I, [P, Z, P, P, Z, I, I, I, I, I] + DROP + [P]),
     "dsvg_attn_bwd": (I, [P, Z, P, P, Z, P, Z, I, I, I, I, I, F] + DROP + [P]),
+    "dsvg_decode_embed": (I, [P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, I, P]),
+    "dsvg_decode_attn": (I, [P, P, Z, P, P, Z, P, P, Z, I, I, I, I, P]),
+    "dsvg_decode_sample": (I, [P, P, I, P, I, P, P, P, P, P, P, I, I, I, I, I, P]),
     "dsvg_ce_args": (I, [P, I, P, P, P, P, Z, I, P, I, I, I, I, P]),
     "dsvg_ce_cmd": (I, [P, P, P, P, P, P, Z, I, P, I, I, I, P]),
     "dsvg_ce_vis": (I, [P, P, P, Z, I, P, I, F, P]),

@@ -266,6 +266,8 @@ class SVGTransformer(nn.Module):
         self._sites = {}
         self._wcache = {}
         self._eps_override = None      # tests inject the VAE noise here (SURVEY.md 8c hazard 2)
+        self._ds = None                # the one live _DecodeState (cached autoregressive decoding)
+        self._decode_hook = None       # tests: called as hook(t, cmd_logits [N, 7], args_logits [N, 11 * C]) after each step
 
     # -------------------------------------------------------------------------------------------------
     def _param(self, name):
@@ -418,7 +420,9 @@ class SVGTransformer(nn.Module):
             return torch.distributions.Categorical(logits=logits / temperature).sample()
 
         if self.autoregressive:
-            return self._greedy_sample_autoregressive(commands_enc, args_enc, label, z, pick, concat_groups)
+            if self.training:
+                return self._greedy_sample_autoregressive(commands_enc, args_enc, label, z, pick, concat_groups)
+            return self._greedy_sample_cached(commands_enc, args_enc, label, z, temperature, concat_groups)
         res = self.forward(commands_enc, args_enc, commands_dec, args_dec, label=label, z=z,
                            hierarch_logits=hierarch_logits, return_tgt=False)
 
@@ -436,8 +440,10 @@ class SVGTransformer(nn.Module):
         return commands_y, args_y
 
     def _greedy_sample_autoregressive(self, commands_enc, args_enc, label, z, pick, concat_groups):
-        """model.py:428-448: token-by-token decoding -- every step re-runs the causal decoder on the prefix (the reference does
-        the same; there is no KV cache in either), keeps the last position's tokens, and feeds them back."""
+        """model.py:428-448 in train mode: token-by-token decoding that re-runs the causal decoder on the whole prefix at
+        every step, as the reference does, keeps the last position's tokens, and feeds them back.  The reference's loop
+        draws fresh dropout masks over the whole prefix at every step, so earlier positions' keys and values change from
+        step to step and a cache cannot reproduce it; eval mode runs _greedy_sample_cached instead."""
         cfg = self.cfg
         if z is None:
             z = self.forward(commands_enc, args_enc, None, None, label=label, encode_mode=True)      # (1, 1, N, dz)
@@ -453,6 +459,11 @@ class SVGTransformer(nn.Module):
             commands_y = torch.cat([commands_y, c_new[..., -1:]], dim=-1)
             args_y = torch.cat([args_y, a_new[..., -1:, :]], dim=-2)
         commands_y, args_y = commands_y[..., 1:], args_y[..., 1:, :]                                 # discard SOS
+        return self._autoregressive_output(commands_y, args_y, concat_groups)
+
+    def _autoregressive_output(self, commands_y, args_y, concat_groups):
+        """Decoded tokens (N, 1, T[, 11]) in the classes the heads predict -> the public result (model.py:440-448)."""
+        cfg = self.cfg
         if self.rel_targets:
             args_y = self._make_absolute(commands_y, args_y)
         if concat_groups:
@@ -461,6 +472,118 @@ class SVGTransformer(nn.Module):
             commands_y = commands_y[keep].reshape(n, -1)
             args_y = args_y[keep].reshape(n, -1, cfg.n_args)
         return commands_y, args_y
+
+    # -------------------------------------------------------------------------------------------------
+    # cached autoregressive decoding (eval mode): csrc/decode.cu
+    # -------------------------------------------------------------------------------------------------
+    def _greedy_sample_cached(self, commands_enc, args_enc, label, z, temperature, concat_groups):
+        """model.py:428-448 with key/value caches.  Position t's decoder output depends on tokens <= t only (causal mask),
+        so each step embeds the one new token per sequence, pushes that row through the stack (attention over the cached
+        keys and values of positions 0..t) and samples the next tokens on the device: max_total_len steps of N rows instead
+        of prefixes of up to max_total_len rows.  With self.graphs, one step is captured as a CUDA graph and replayed.
+
+        Device memory of the caches: n_layers_decode * N * max_total_len * 2 d_model * planes * 2 bytes (4 layers, N = 512,
+        max_total_len 139, d_model 256, two planes: 0.58 GB), plus N * max_total_len * 12 int64 tokens."""
+        cfg = self.cfg
+        if z is None:
+            z = self.forward(commands_enc, args_enc, None, None, label=label, encode_mode=True)       # (1, 1, N, dz)
+            z = z.permute(2, 0, 1, 3)                                                                 # batch-first
+        if not z.is_cuda:
+            raise RuntimeError("deepsvg_b200 has no CPU path: inputs and parameters must live on a CUDA device")
+        N, dev, T = z.shape[0], z.device, cfg.max_total_len
+        if cfg.label_condition:
+            if label is None:
+                raise ValueError("label_condition=True needs `label`")
+            label = label.to(device=dev, dtype=torch.long).contiguous().view(-1)
+            if label.numel() != N:
+                raise ValueError("label must hold one class id per icon (%d), got %d" % (N, label.numel()))
+        key = (N, self.planes, str(dev), hash(tuple(self._param(n).data_ptr() for n in self._pnames)))
+        st = self._ds
+        if st is None or st.key != key:
+            self._ds = None                       # at most one set of caches and one decode graph pool alive
+            st = self._ds = _DecodeState(self, key, N, dev)
+        # ---- per call: weight operands, folded embedding table, per-layer row vectors, sampling parameters ----
+        P = self._param
+        sv = st.sv
+        for name in st.weights:
+            self._pack(name)
+        ops.embed_fold(P("decoder.embedding.arg_embed.weight"), P("decoder.embedding.embed_fcn.weight"),
+                       P("decoder.embedding.embed_fcn.bias"), st.table, st.base, self.args_dim, cfg.n_args, cfg.d_model)
+        z_act = Act(N, cfg.dim_z, self.planes, dev)
+        ops.cast_act(z.reshape(N, cfg.dim_z).contiguous().float(), N, cfg.dim_z, out=z_act)
+        lab_d = None
+        if cfg.label_condition:
+            lab_d = Act(N, cfg.dim_label, self.planes, dev)
+            ops.gather_rows(P("decoder.label_embedding.label_embedding.weight"), label, N, cfg.dim_label, lab_d)
+        for i, rv in enumerate(st.rowvec):                           # improved_transformer.py:131-136, fixed over the steps
+            rv.copy_(self._globals_fwd(sv, "decoder.decoder.layers.%d" % i, z_act, N, lab_d, 1))
+        st.temperature.fill_(float(temperature))
+        if temperature >= 1e-3:
+            st.seed.random_()                                         # torch's CUDA generator: manual_seed reproduces a run
+        st.step.zero_()
+        hook = self._decode_hook
+        t = 0
+        if self.graphs and not st.graph_failed and st.graph is None:
+            self._decode_step(st)                  # step 0 eagerly: also configures every kernel on this device
+            if hook is not None:
+                hook(0, st.cmd_logits, st.args_logits)
+            t = 1
+            try:
+                torch.cuda.synchronize(dev)
+                g = torch.cuda.CUDAGraph()
+                from . import _lib
+                n0 = _lib.launch_count()
+                with torch.cuda.graph(g, pool=st.pool):
+                    self._decode_step(st)
+                st.graph, st.n_launches = g, _lib.launch_count() - n0
+            except Exception as e:                   # capture is an optimisation: fall back to eager launches
+                import sys
+                sys.stderr.write("deepsvg_b200: WARNING: CUDA-graph capture of the decode step failed (%r); running "
+                                 "eagerly\n" % (e,))
+                st.graph, st.graph_failed = None, True
+        for t in range(t, T):
+            if self.graphs and st.graph is not None:
+                st.graph.replay()
+                self.graph_kernel_launches += st.n_launches
+            else:
+                self._decode_step(st)
+            if hook is not None:
+                hook(t, st.cmd_logits, st.args_logits)
+        commands_y = st.out_cmd.view(N, 1, T).clone()
+        args_y = st.out_args.view(N, 1, T, cfg.n_args).clone()
+        return self._autoregressive_output(commands_y, args_y, concat_groups)
+
+    def _decode_step(self, st):
+        """One decode step on the state's static buffers: embed -> layers -> final LayerNorm -> heads -> sample, t += 1."""
+        cfg = self.cfg
+        P = self._param
+        N, T, dev, pl = st.N, cfg.max_total_len, st.dev, self.planes
+        d, H, nl = cfg.d_model, cfg.n_heads, cfg.n_layers_decode
+        hd = d // H
+        x = torch.empty(N, d, device=dev)
+        ops.decode_embed(st.step, st.cmd_in, st.args_in, st.grp, st.key_valid, P("decoder.embedding.command_embed.weight"),
+                         st.table, st.base, P("decoder.embedding.pos_encoding.pos_embed.weight"),
+                         P("decoder.embedding.group_embed.weight"), x, N, T, self.args_dim, cfg.n_args, d)
+        nxt = None
+        for i in range(nl):
+            lp = "decoder.decoder.layers.%d" % i
+            nm = "decoder.decoder.layers.%d.norm1" % (i + 1) if i + 1 < nl else "decoder.decoder.norm"
+            attn = (lambda qkv, o, i=i: ops.decode_attn(st.step, qkv, st.k_cache[i], st.v_cache[i], st.key_valid, o, N, H,
+                                                        hd, T))
+            x, nxt = self._layer_fwd(st.sv, lp, x, N, 1, N, None, st.rowvec[i], 1, a_pre=nxt,
+                                     next_ln=(P(nm + ".weight"), P(nm + ".bias")), attn=attn)
+        if nxt is not None:
+            y = nxt[0]
+        else:
+            y = Act(N, d, pl, dev)
+            ops.ln_fwd(x, P("decoder.decoder.norm.weight"), P("decoder.decoder.norm.bias"), y, torch.empty(N, device=dev),
+                       torch.empty(N, device=dev), N, d)
+        w, _ = self._pack("decoder.fcn.command_fcn.weight")
+        ops.linear(y, w, N, cfg.n_commands, d, bias=P("decoder.fcn.command_fcn.bias"), out_f32=st.cmd_logits)
+        w, _ = self._pack("decoder.fcn.args_fcn.weight")
+        ops.linear(y, w, N, cfg.n_args * self.args_dim, d, bias=P("decoder.fcn.args_fcn.bias"), out_f32=st.args_logits)
+        ops.decode_sample(st.step, st.cmd_logits, st.args_logits, st.temperature, st.seed, st.cmd_in, st.args_in,
+                          st.out_cmd, st.out_args, N, T, cfg.n_args, self.args_dim)
 
     def _make_absolute(self, commands_y, args_y):
         """model.py:461-478: relative argument classes back to absolute coordinates (running sum of the end positions over
@@ -522,10 +645,11 @@ class SVGTransformer(nn.Module):
         # bit 31 of the site: `seed` is a device pointer (include/dsvg_b200.h, DSVG_SEED_IS_DEVICE_PTR)
         return (self.cfg.dropout if p is None else p, self._site(tag) | 0x80000000, sv.seed_ptr)
 
-    def _layer_fwd(self, sv, pre, x, M, L, nseq, key_valid, rowvec, rpg, a_pre=None, next_ln=None):
+    def _layer_fwd(self, sv, pre, x, M, L, nseq, key_valid, rowvec, rpg, a_pre=None, next_ln=None, attn=None):
         """One pre-LN block.  a_pre = (LN1(x) Act, mean, rstd) when the previous GEMM already produced it in its epilogue;
         next_ln = (gamma, beta) of the LayerNorm that consumes this block's output (next layer's norm1 or the stack's final
-        norm): when the GEMM tile owns whole rows (ops.ln_fusable) it is computed in the FFN2 epilogue and returned."""
+        norm): when the GEMM tile owns whole rows (ops.ln_fusable) it is computed in the FFN2 epilogue and returned.
+        attn(qkv, o), when given, replaces the self-attention over whole sequences (the cached decoder's one-row step)."""
         cfg = self.cfg
         d, ff, H = cfg.d_model, cfg.dim_feedforward, cfg.n_heads
         hd = d // H
@@ -544,8 +668,11 @@ class SVGTransformer(nn.Module):
         ops.linear(a, w_in, M, 3 * d, d, bias=P("self_attn.in_proj_bias"), scale_cols=d, scale=float(hd) ** -0.5,
                    out_act=qkv)
         o = Act(M, d, pl, dev)
-        ops.attn_fwd(qkv, key_valid, o, nseq, L, H, hd, self._drop(sv, pre + ".attn"),
-                     causal=pre.startswith(getattr(sv, "causal_stack", "\0")))
+        if attn is not None:
+            attn(qkv, o)
+        else:
+            ops.attn_fwd(qkv, key_valid, o, nseq, L, H, hd, self._drop(sv, pre + ".attn"),
+                         causal=pre.startswith(getattr(sv, "causal_stack", "\0")))
         x1 = torch.empty(M, d, device=dev)
         w_o, _ = self._pack(pre + ".self_attn.out_proj.weight")
         b = Act(M, d, pl, dev)
@@ -1223,7 +1350,9 @@ class SVGTransformer(nn.Module):
                 hash(ptrs))
 
     def release_graphs(self):
-        """Drops the captured step (and its private memory pool: activations of one step)."""
+        """Drops the captured step (and its private memory pool: activations of one step), and the decode caches and
+        captured decode step of greedy_sample."""
+        self._ds = None
         gs, self._gs = self._gs, None
         self._gs_streak = (None, 0)
         if gs is not None:
@@ -1388,3 +1517,42 @@ class _GraphState:
             res.append(out[off:off + p.numel()].view(p.shape))
             off += p.numel()
         return res
+
+
+class _DecodeState:
+    """Static buffers of cached decoding for one (N, precision, device, parameter storage): per-layer key/value caches, the
+    step counter, token and bookkeeping buffers, the per-call refreshed inputs (folded embedding table, row vectors,
+    temperature, seed), the head logits, and the captured decode step with its private memory pool."""
+
+    def __init__(self, model, key, N, dev):
+        cfg = model.cfg
+        T, d, H, pl = cfg.max_total_len, cfg.d_model, cfg.n_heads, model.planes
+        na, V = cfg.n_args, model.args_dim
+        self.key, self.N, self.dev = key, N, dev
+        self.sv = _Saved()
+        self.sv.training = False
+        self.step = torch.zeros(2, dtype=torch.int32, device=dev)            # t, block ticket
+        self.cmd_in = torch.zeros(N, dtype=torch.int32, device=dev)
+        self.args_in = torch.zeros(N, na, dtype=torch.int32, device=dev)
+        self.grp = torch.zeros(N, dtype=torch.int32, device=dev)
+        self.key_valid = torch.zeros(N, T, dtype=torch.uint8, device=dev)
+        self.out_cmd = torch.zeros(N, T, dtype=torch.int64, device=dev)
+        self.out_args = torch.zeros(N, T, na, dtype=torch.int64, device=dev)
+        self.k_cache = [ops.decode_cache(N, H, d // H, T, pl, dev) for _ in range(cfg.n_layers_decode)]
+        self.v_cache = [ops.decode_cache(N, H, d // H, T, pl, dev) for _ in range(cfg.n_layers_decode)]
+        self.table = torch.empty(na * V, d, device=dev)
+        self.base = torch.empty(d, device=dev)
+        self.rowvec = [torch.empty(N, d, device=dev) for _ in range(cfg.n_layers_decode)]
+        self.temperature = torch.zeros(1, device=dev)
+        self.seed = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.cmd_logits = torch.empty(N, cfg.n_commands, device=dev)
+        self.args_logits = torch.empty(N, na * V, device=dev)
+        self.weights = ["decoder.fcn.command_fcn.weight", "decoder.fcn.args_fcn.weight"]
+        for i in range(cfg.n_layers_decode):
+            lp = "decoder.decoder.layers.%d." % i
+            self.weights += [lp + n for n in ("self_attn.in_proj_weight", "self_attn.out_proj.weight", "linear1.weight",
+                                              "linear2.weight", "linear_global.weight")]
+            if cfg.label_condition:
+                self.weights.append(lp + "linear_global2.weight")
+        self.pool = torch.cuda.graph_pool_handle()
+        self.graph, self.graph_failed, self.n_launches = None, False, 0

@@ -223,6 +223,35 @@ def attn_bwd(qkv, key_valid, dout, dqkv, nseq, L, H, hd, q_scale, drop, causal=F
     _lib.check(rc, "dsvg_attn_bwd")
 
 
+def decode_embed(step, cmd_in, args_in, grp, key_valid, cmd_tab, table, base, pos_tab, grp_tab, x, N, Tmax, V, n_args, d):
+    rc = _lib.load().dsvg_decode_embed(step.data_ptr(), cmd_in.data_ptr(), args_in.data_ptr(), grp.data_ptr(),
+                                       key_valid.data_ptr(), cmd_tab.data_ptr(), table.data_ptr(), base.data_ptr(),
+                                       pos_tab.data_ptr(), grp_tab.data_ptr(), x.data_ptr(), N, Tmax, V, n_args, d, _stream())
+    _lib.check(rc, "dsvg_decode_embed")
+
+
+def decode_cache(N, H, hd, Tmax, planes, device):
+    """One layer's key or value cache: bf16 [planes, N, H, Tmax, hd] (the lo plane after the hi plane)."""
+    return torch.empty(planes, N, H, Tmax, hd, dtype=BF16, device=device)
+
+
+def decode_attn(step, qkv, k_cache, v_cache, key_valid, out, N, H, hd, Tmax):
+    """k_cache / v_cache from decode_cache(); qkv, out: Act with the caches' plane count."""
+    lo = k_cache[0].numel() if k_cache.shape[0] == 2 else 0
+    rc = _lib.load().dsvg_decode_attn(step.data_ptr(), qkv.ptr, qkv.lo, k_cache.data_ptr(), v_cache.data_ptr(), lo,
+                                      key_valid.data_ptr(), out.ptr, out.lo, N, H, hd, Tmax, _stream())
+    _lib.check(rc, "dsvg_decode_attn")
+
+
+def decode_sample(step, cmd_logits, args_logits, temperature, seed, cmd_in, args_in, out_cmd, out_args, N, Tmax, n_args,
+                  n_classes):
+    rc = _lib.load().dsvg_decode_sample(step.data_ptr(), cmd_logits.data_ptr(), cmd_logits.stride(0),
+                                        args_logits.data_ptr(), args_logits.stride(0), temperature.data_ptr(),
+                                        seed.data_ptr(), cmd_in.data_ptr(), args_in.data_ptr(), out_cmd.data_ptr(),
+                                        out_args.data_ptr(), N, Tmax, cmd_logits.shape[1], n_args, n_classes, _stream())
+    _lib.check(rc, "dsvg_decode_sample")
+
+
 def ce_args(logits, ld_logits, commands, args, counts, dl, acc, nseq, L, n_args, n_classes):
     rc = _lib.load().dsvg_ce_args(logits.data_ptr(), ld_logits, commands.data_ptr(), args.data_ptr(),
                                   counts.data_ptr(), dl.ptr, dl.lo, dl.ld, acc.data_ptr(), nseq, L, n_args, n_classes,

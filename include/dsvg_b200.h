@@ -193,6 +193,33 @@ int dsvg_attn_bwd(const dsvg_bf16* qkv, size_t qkv_lo_off, const uint8_t* key_va
                   size_t dout_lo_off, dsvg_bf16* dqkv, size_t dqkv_lo_off, int nseq, int L, int H, int head_dim, int causal,
                   float q_scale, float drop_p, uint32_t drop_site, uint64_t seed, void* stream);
 
+/* ---- incremental autoregressive decoding (SVGTransformer._greedy_sample / greedy_sample, model.py:428-448) --------
+ * One new row per sequence per step over per-layer key/value caches.  `step` is a DEVICE int[2]: step[0] = t, the position
+ * being decoded, step[1] = 0 (a block ticket); the caller zeroes both before step 0, dsvg_decode_sample advances step[0].
+ * Every entry point reads t from there, so one captured CUDA graph of a whole step replays for every t. */
+/* SVGEmbedding (model.py:46-57, use_group=True) of the token at position t into x[N, d]: SOS with PAD arguments at t = 0
+ * (model.py:428), else cmd_in[N] / args_in[N, n_args].  Same table, base and sum order as dsvg_embed_fwd.  Also carries
+ * the bookkeeping of dsvg_seq_prep (model/utils.py:7-17, 35-42) over from t - 1: grp[N] = number of "m" in 0..t,
+ * key_valid[n * Tmax + t] = no EOS in 0..t. */
+int dsvg_decode_embed(const int* step, const int* cmd_in, const int* args_in, int* grp, uint8_t* key_valid,
+                      const float* cmd_tab, const float* table, const float* base, const float* pos_tab, const float* grp_tab,
+                      float* x, int N, int Tmax, int V, int n_args, int d, void* stream);
+/* Causal self-attention of row t (functional.py:168-248 with square_subsequent_mask and key_padding_mask, model.py:269):
+ * appends K and V of qkv[N, 3d] (q pre-scaled) to k_cache / v_cache [N, H, Tmax, head_dim] at position t (every plane;
+ * the lo plane cache_lo_off elements after the first), then out[N, d] = softmax(q K^T over valid keys 0..t) V in fp32.
+ * qkv, the caches and out have one plane each or two each.  Tmax <= 256. */
+int dsvg_decode_attn(const int* step, const dsvg_bf16* qkv, size_t qkv_lo_off, dsvg_bf16* k_cache, dsvg_bf16* v_cache,
+                     size_t cache_lo_off, const uint8_t* key_valid, dsvg_bf16* out, size_t out_lo_off, int N, int H,
+                     int head_dim, int Tmax, void* stream);
+/* Token choice of step t (model.py:415-418 pick() + _make_valid, :450-459): *temperature < 1e-3 takes the argmax of the
+ * n_cmd command logits and of each argument slot's n_classes logits (ties to the lowest index); otherwise Gumbel-max with
+ * noise from a counter hash of (*seed, t, sequence, slot, class).  Argument slots CMD_ARGS_MASK marks unused become -1,
+ * the others class - 1.  Writes out_cmd[n * Tmax + t], out_args[(n * Tmax + t) * n_args + k] and the next step's
+ * cmd_in / args_in, then step[0] = t + 1. */
+int dsvg_decode_sample(int* step, const float* cmd_logits, int ld_cmd, const float* args_logits, int ld_args,
+                       const float* temperature, const unsigned long long* seed, int* cmd_in, int* args_in, long long* out_cmd,
+                       long long* out_args, int N, int Tmax, int n_cmd, int n_args, int n_classes, void* stream);
+
 /* ---- SVGLoss (model/loss.py:19-65): loss sums + unit-scale d(loss)/d(logits) --------------------------- */
 int dsvg_ce_args(const float* logits, int ld_logits, const float* commands, const float* args, const float* counts,
                  dsvg_bf16* dlogits, size_t dl_lo_off, int ld_dl, float* acc, int nseq, int L, int n_args,
