@@ -1283,11 +1283,12 @@ __device__ __forceinline__ void outer_chunk(const float (&a)[2][16], uint32_t st
 }
 
 // ------------------------------------------------------------------------------------------------
-// dsvg_outer kernel (MN-major operands): one output tile [128 x BQ] per CTA, contraction over an M range
+// dsvg_outer kernel (MN-major operands): output tiles [128 x BQ], each a sum of contractions over row ranges (chunks)
 // ------------------------------------------------------------------------------------------------
 // Warpgroup g (warps 4 g .. 4 g + 3) accumulates all 128 P rows (two m64 halves) against Q columns
 // [g BQ / 2, (g + 1) BQ / 2) in registers; warpgroup 0 also sums the A columns (bias gradient) with an n8 wgmma
-// against an all-ones operand.  The last warp is the TMA producer.
+// against an all-ones operand.  The last warp is the TMA producer.  Single-plane operands run persistent CTAs over
+// (tile, chunk) work items (outer_persistent); two-plane operands one (tile, chunk) per CTA (outer_body).
 template <int BQ, int NPLANES>
 struct OuterCfg {
   static constexpr int kBoxBytes = 64 * 64 * 2;                 // [64 rows(m) x 64 cols] = 8 KB
@@ -1296,17 +1297,21 @@ struct OuterCfg {
   static constexpr int kStageBytes = NPLANES * (kABytes + kBBytes);
   static constexpr int kStages = (NPLANES == 1) ? 4 : 2;
   static constexpr int kOnesBytes = 1024;   // [8 x 64] bf16 1.0, K-major B operand of the column-sum wgmma
-  // 8 consumer warps.  Their transposition buffers alias the operand stages: the epilogue starts once every consumer
-  // warp has retired its last wgmma, and by then every TMA load has landed.
+  // 8 consumer warps.  In the two-plane kernel their transposition buffers alias the operand stages: the epilogue starts
+  // once every consumer warp has retired its last wgmma, and by then every TMA load has landed.
   static constexpr int kEpiWarps = 8;
-  static constexpr int kThreads = 32 * kEpiWarps + 32;
+  // one producer warp; the persistent single-plane kernel gives it a whole warpgroup, to hand the consumers its registers
+  static constexpr int kThreads = 32 * kEpiWarps + (NPLANES == 1 ? 128 : 32);
   static constexpr int kNW = BQ / 2;   // Q columns per warpgroup
   static_assert(kEpiWarps * kStageWarpBytes <= kStages * kStageBytes, "outer: staging must fit in the operand stages");
-  static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kOnesBytes + 256;
+  // + the persistent kernel's 16-row staging tile per consumer warp
+  static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kOnesBytes + 256 +
+                                    (NPLANES == 1 ? kEpiWarps * kStageWarpBytes / 2 : 0);
+  static_assert(kSmemBytes <= 227 * 1024, "outer: shared memory over the per-block limit of sm_90");
 };
 
-// The whole CTA program; `tile_id` / `split_id` select the output tile and the M range (the block indices of the single-problem
-// kernel, a table lookup in the grouped one).  The tensor maps live in kernel-parameter space (__grid_constant__) of the caller.
+// The whole CTA program of the two-plane kernel; `tile_id` / `split_id` (the block indices) select the output tile and the
+// M range.  The tensor maps live in kernel-parameter space (__grid_constant__) of the caller.
 template <int BQ, int NPLANES>
 __device__ __forceinline__ void outer_body(const CUtensorMap* tmA_p, const CUtensorMap* tmAlo_p, const CUtensorMap* tmB_p,
                                            const CUtensorMap* tmBlo_p, int M, int P, int Q, int mblk_per_split, float alpha,
@@ -1465,39 +1470,236 @@ __device__ __forceinline__ void outer_body(const CUtensorMap* tmA_p, const CUten
   }
 }
 
-template <int BQ, int NPLANES>
-__global__ void __launch_bounds__((OuterCfg<BQ, NPLANES>::kThreads), 1)
-outer_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmAlo,
-             const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmBlo, int M, int P, int Q,
-             int mblk_per_split, float alpha, const float* alpha_dev, float* C, int ldc, float* colsum_out,
-             uint32_t lbo, uint32_t sbo, int vec) {
-  outer_body<BQ, NPLANES>(&tmA, &tmAlo, &tmB, &tmBlo, M, P, Q, mblk_per_split, alpha, alpha_dev, C, ldc, colsum_out, lbo, sbo,
-                          vec, int(blockIdx.x), int(blockIdx.y));
-}
-
-// Grouped launch: the weight gradients of one transformer block (QKV, out-proj, FFN1, FFN2: same row count M, different
-// operands) share ONE wave of CTAs.  Launched one by one, each of them splits its M range many ways to fill the machine and
-// pays the red.add traffic and a pipeline ramp per launch for a small result; together they split the M range fewer ways
-// and every CTA streams a longer run of row blocks.  128 x 256 tiles throughout.
+// The problems of one launch: a single dsvg_outer call, or the weight gradients of one transformer block (QKV, out-proj,
+// FFN1, FFN2: same row count M, different operands) from dsvg_outer_group, which then share one persistent grid instead of
+// paying a pipeline ramp and a ragged last wave per launch.  Work item w of the single-plane kernel is (chunk w / T,
+// tile w % T), T = tile_begin[n] output tiles of 128 x BQ over all problems, a chunk = mblk_per_chunk row blocks of 64 rows.
 constexpr int kMaxGroup = 4;
 struct OuterGroup {
   CUtensorMap a[kMaxGroup];
   CUtensorMap b[kMaxGroup];
+  CUtensorMap alo, blo;            // two-plane launches (always one problem): the low planes of a[0] / b[0]
   float* C[kMaxGroup];
   float* colsum[kMaxGroup];
   const float* alpha_dev[kMaxGroup];
   float alpha[kMaxGroup];
   int P[kMaxGroup], Q[kMaxGroup], ldc[kMaxGroup], vec[kMaxGroup];
-  int cta_begin[kMaxGroup + 1];   // first CTA of each problem (tiles x splits CTAs per problem)
-  int n, M, splits, mblk_per_split;
+  int tile_begin[kMaxGroup + 1];   // first output tile of each problem; tile_begin[n] = T
+  int n, M, chunks, mblk_per_chunk;
 };
-__global__ void __launch_bounds__((OuterCfg<256, 1>::kThreads), 1)
-outer_group_kernel(const __grid_constant__ OuterGroup g, uint32_t lbo, uint32_t sbo) {
-  int p = 0;
-  while (p + 1 < g.n && int(blockIdx.x) >= g.cta_begin[p + 1]) ++p;
-  const int local = int(blockIdx.x) - g.cta_begin[p];
-  outer_body<256, 1>(&g.a[p], &g.a[p], &g.b[p], &g.b[p], g.M, g.P[p], g.Q[p], g.mblk_per_split, g.alpha[p], g.alpha_dev[p],
-                          g.C[p], g.ldc[p], g.colsum[p], lbo, sbo, g.vec[p], local / g.splits, local % g.splits);
+
+// One 64-row half of a consumer warp's accumulators (P rows prow + [0, 16)) -> C[row, col0 + ...] += alpha * acc, in
+// 32-column chunks through the warp's 16-row staging tile: eight lanes then cover one 128-byte row segment with 16-byte
+// reductions (ldc % 4 == 0, Q % 4 == 0 and a 16-byte aligned C), or 32 lanes one with scalar ones (gradient slices at odd
+// offsets of a flat bucket).  Straight from the fragments, a reduction instruction would touch 16 rows (measured slower
+// where the reductions are not hidden behind long row chunks: 4096-row weight gradients).
+template <int NV>
+__device__ __forceinline__ void outer_red_half(const float (&acc)[NV], uint32_t stage_addr, int lane, int prow, int col0, int P,
+                                               int Q, float alpha, float* C, int ldc, int vec) {
+#pragma unroll
+  for (int cc = 0; cc < NV / 16; ++cc) {
+    if (col0 + 32 * cc >= Q) break;   // warp-uniform
+    __syncwarp();
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int lr = 8 * i + (lane >> 2), col = 8 * j + 2 * (lane & 3);
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stage_addr + (lr * kStageRow + col) * 4),
+                     "f"(acc[16 * cc + 4 * j + 2 * i]), "f"(acc[16 * cc + 4 * j + 2 * i + 1]) : "memory");
+      }
+    __syncwarp();
+    if (vec) {
+      const int cg = lane & 7, col = col0 + 32 * cc + 4 * cg;
+#pragma unroll
+      for (int it = 0; it < 4; ++it) {
+        const int lr = (lane >> 3) + 4 * it;
+        const float4 x = ld_shared_v4(stage_addr + (lr * kStageRow + 4 * cg) * 4);
+        if (prow + lr < P && col < Q)
+          red_add_v4(C + size_t(prow + lr) * ldc + col, x.x * alpha, x.y * alpha, x.z * alpha, x.w * alpha);
+      }
+    } else {
+      const int col = col0 + 32 * cc + lane;
+#pragma unroll 4
+      for (int lr = 0; lr < 16; ++lr) {
+        const float x = ld_shared_f32(stage_addr + (lr * kStageRow + lane) * 4);
+        if (prow + lr < P && col < Q) atomicAdd(C + size_t(prow + lr) * ldc + col, x * alpha);
+      }
+    }
+  }
+  __syncwarp();
+}
+
+// Single-plane operands: a persistent grid (at most one CTA per SM) walks the launch's work items in chunk-major order, so
+// the CTAs that read the same rows of a shared operand (the same A for the Q tiles of one P range, the same B for the P
+// tiles) stream them at about the same time and L2 serves all but the first read.  Each output element is still the sum of
+// per-chunk fp32 wgmma chains of at most kMaxSplitBlocks row blocks, added with red.add.  The producer warp runs ahead into
+// the next item's row blocks while the consumer warps reduce the current one from their registers.
+template <int BQ>
+__device__ __forceinline__ void outer_persistent(const OuterGroup& g, uint32_t lbo, uint32_t sbo) {
+  using Cfg = OuterCfg<BQ, 1>;
+  constexpr int kNW = Cfg::kNW;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* tiles = smem;
+  uint8_t* ones = smem + Cfg::kStages * Cfg::kStageBytes;  // 1024-aligned
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ones + Cfg::kOnesBytes);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + Cfg::kStages;
+  uint8_t* staging = reinterpret_cast<uint8_t*>(bars) + 256;   // the consumer warps' own, the stages stay in flight
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  constexpr int kProducer = Cfg::kEpiWarps;
+
+  if (warp == kProducer && lane == 0) {
+    for (int s = 0; s < Cfg::kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], Cfg::kEpiWarps);
+    }
+    fence_barrier_init();
+  }
+  for (int i = threadIdx.x; i < Cfg::kOnesBytes / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(ones)[i] = 0x3F803F80u;
+  fence_proxy_async_smem();
+  __syncthreads();
+  pdl_wait();   // everything above touched only this CTA's shared memory
+
+  const int T = g.tile_begin[g.n];
+  const int items = T * g.chunks;
+  const int total_mblk = (g.M + 63) / 64;
+  // work item -> problem p, output tile origin (p0, q0), row blocks [mb_begin, mb_end)
+  auto decode = [&](int w, int& p, int& p0, int& q0, int& mb_begin, int& mb_end) {
+    const int chunk = w / T;
+    int t = w - chunk * T;
+    p = 0;
+    while (p + 1 < g.n && t >= g.tile_begin[p + 1]) ++p;
+    t -= g.tile_begin[p];
+    const int q_tiles = (g.Q[p] + BQ - 1) / BQ;
+    p0 = (t / q_tiles) * 128;
+    q0 = (t % q_tiles) * BQ;
+    mb_begin = chunk * g.mblk_per_chunk;
+    mb_end = min(total_mblk, mb_begin + g.mblk_per_chunk);
+  };
+
+  if (warp >= kProducer) {
+    // producer warpgroup: registers go to the consumers (40 x 128 + 232 x 256 = 64512), one warp issues
+    setmaxnreg_dec<40>();
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int w = blockIdx.x; w < items && warp == kProducer; w += gridDim.x) {
+      // the next kernel may launch once every CTA is on its last item: earlier, its CTAs would only wait for SMs
+      if (w + int(gridDim.x) >= items) pdl_launch_dependents();
+      int p, p0, q0, mb_begin, mb_end;
+      decode(w, p, p0, q0, mb_begin, mb_end);
+      for (int mb = mb_begin; mb < mb_end; ++mb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        if (elect_one()) {
+          uint8_t* st = tiles + stage * Cfg::kStageBytes;
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+#pragma unroll
+          for (int i = 0; i < 2; ++i) tma_load_2d(st + i * Cfg::kBoxBytes, &g.a[p], &full_bar[stage], p0 + 64 * i, mb * 64);
+#pragma unroll
+          for (int j = 0; j < BQ / 64; ++j)
+            tma_load_2d(st + Cfg::kABytes + j * Cfg::kBoxBytes, &g.b[p], &full_bar[stage], q0 + 64 * j, mb * 64);
+        }
+        __syncwarp();
+        if (++stage == Cfg::kStages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+    }
+    return;
+  }
+
+  setmaxnreg_inc<232>();
+  const uint32_t stage_buf = smem_u32(staging) + warp * (kStageWarpBytes / 2);
+  const int quarter = warp & 3;   // warp within its warpgroup: P rows [16 quarter, +16) of each m64 half
+  const int half = warp >> 2;     // warpgroup: Q columns [half * kNW, (half + 1) * kNW)
+  const uint64_t ones_desc = gmma_smem_desc(smem_u32(ones), 16, 1024);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int w = blockIdx.x; w < items; w += gridDim.x) {
+    if (w + int(gridDim.x) >= items) pdl_launch_dependents();
+    int p, p0, q0, mb_begin, mb_end;
+    decode(w, p, p0, q0, mb_begin, mb_end);
+    float acc[2][kNW / 2];
+    float cs[2][4];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int j = 0; j < kNW / 2; ++j) acc[h][j] = 0.f;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) cs[h][j] = 0.f;
+    }
+    int prev_stage = 0;
+    for (int mb = mb_begin; mb < mb_end; ++mb) {
+      mbar_wait(&full_bar[stage], phase);
+      wgmma_fence();
+      const uint32_t a_hi = smem_u32(tiles + stage * Cfg::kStageBytes);
+      const uint32_t b_hi = a_hi + Cfg::kABytes + half * (kNW / 64) * Cfg::kBoxBytes;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {  // 16 rows (= 2 KB) of the 64-row block per k16 step
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t ao = h * Cfg::kBoxBytes + k * 2048;
+          wgmma_m64_tt<kNW>(acc[h], gmma_smem_desc(a_hi + ao, lbo, sbo), gmma_smem_desc(b_hi + k * 2048, lbo, sbo));
+          // issued unconditionally (a wgmma under a run-time branch makes ptxas serialise all of them, C7520); only
+          // warpgroup 0 of an item on the first Q tile writes the sums out
+          wgmma_m64n8_tk(cs[h], gmma_smem_desc(a_hi + ao, lbo, sbo), ones_desc);
+        }
+      }
+      wgmma_commit();
+      if (mb > mb_begin) {
+        wgmma_wait<1>();
+        if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      }
+      prev_stage = stage;
+      if (++stage == Cfg::kStages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      wgmma_fence_regs(acc[h]);
+      wgmma_fence_regs(cs[h]);
+    }
+    if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);   // the producer refills it for the next item during the reduction
+
+    const int P = g.P[p], Q = g.Q[p];
+    float alpha = g.alpha[p];
+    if (g.alpha_dev[p] != nullptr) alpha *= __ldg(g.alpha_dev[p]);
+    const int prow0 = p0 + 16 * quarter;
+    const int col0 = q0 + half * kNW;
+    if (col0 < Q) {   // warp-uniform
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        outer_red_half(acc[h], stage_buf, lane, prow0 + 64 * h, col0, P, Q, alpha, g.C[p], g.ldc[p], g.vec[p]);
+    }
+    if (g.colsum[p] != nullptr && q0 == 0 && half == 0 && (lane & 3) == 0) {
+      // column 0 of the [128 x 8] column-sum tile = sum over this chunk's rows of A[:, p]
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int prow = prow0 + 64 * h + 8 * i + (lane >> 2);
+          if (prow < P) atomicAdd(g.colsum[p] + prow, cs[h][2 * i] * alpha);
+        }
+    }
+  }
+}
+
+template <int BQ, int NPLANES>
+__global__ void __launch_bounds__((OuterCfg<BQ, NPLANES>::kThreads), 1)
+outer_kernel(const __grid_constant__ OuterGroup g, uint32_t lbo, uint32_t sbo) {
+  if constexpr (NPLANES == 1)
+    outer_persistent<BQ>(g, lbo, sbo);
+  else
+    outer_body<BQ, NPLANES>(&g.a[0], &g.alo, &g.b[0], &g.blo, g.M, g.P[0], g.Q[0], g.mblk_per_chunk, g.alpha[0],
+                            g.alpha_dev[0], g.C[0], g.ldc[0], g.colsum[0], lbo, sbo, g.vec[0], int(blockIdx.x),
+                            int(blockIdx.y));
 }
 
 static int sm_count() {
@@ -1611,30 +1813,56 @@ static int pick_mode(const Epi& ep, bool split, int N) {
 // tensor core, and shorter chains keep the weight gradients of long row ranges (M ~ 131072) within 2e-5 of an fp64 sum.
 constexpr int kMaxSplitBlocks = 48;
 
+// Fills g.chunks / g.mblk_per_chunk and launches.  Two-plane: one CTA per (tile, chunk), as many chunks as fill one wave.
+// Single-plane (persistent): the chunk count that minimises the launch's makespan, counted in row blocks per CTA plus one
+// per work item for its reduction, e.g. the hier block's 16 tiles at M = 131072 in 49 chunks of 42 row blocks (784 items,
+// 5.94 per SM) rather than 43 of 48 (688 items, 5.2 per SM: a last round on a fifth of the machine).
 template <int BQ, int NPLANES>
-static int launch_outer(const CUtensorMap& a, const CUtensorMap& alo, const CUtensorMap& b, const CUtensorMap& blo,
-                        int M, int P, int Q, float alpha, const float* alpha_dev, float* C, int ldc, float* colsum_out,
-                        cudaStream_t st) {
+static int launch_outer(OuterGroup& g, cudaStream_t st) {
   using Cfg = OuterCfg<BQ, NPLANES>;
   static bool configured[kMaxDevices] = {};
   if (first_use_on_device(configured)) {
     DSVG_CUDA((cudaFuncSetAttribute(outer_kernel<BQ, NPLANES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     Cfg::kSmemBytes)));
   }
-  const int out_tiles = ceil_div(P, 128) * ceil_div(Q, BQ);
-  const int total_mblk = ceil_div(M, 64);
-  int splits = sm_count() / out_tiles;  // one CTA per SM fits (shared memory): fill exactly one wave, no ragged tail
-  if (splits < ceil_div(total_mblk, kMaxSplitBlocks)) splits = ceil_div(total_mblk, kMaxSplitBlocks);
-  if (splits > total_mblk / 4) splits = total_mblk / 4;       // keep >= 4 blocks of 64 rows per split
-  if (splits < 1) splits = 1;
-  const int per = ceil_div(total_mblk, splits);
-  splits = ceil_div(total_mblk, per);
-  dim3 grid(out_tiles, splits);
-  DSVG_CUDA(launch_k(outer_kernel<BQ, NPLANES>, grid, dim3(Cfg::kThreads), Cfg::kSmemBytes, st, a, alo, b, blo, M, P, Q, per, alpha,
-                     alpha_dev, C, ldc, colsum_out, uint32_t(Cfg::kBoxBytes), 1024u,
-                     int(ldc % 4 == 0 && Q % 4 == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0)));
+  const int tiles = g.tile_begin[g.n];
+  const int total_mblk = ceil_div(g.M, 64);
+  const int min_chunks = ceil_div(total_mblk, kMaxSplitBlocks);
+  const int max_chunks = total_mblk / 4 > min_chunks ? total_mblk / 4 : min_chunks;   // >= 4 blocks of 64 rows per chunk
+  dim3 grid;
+  if (NPLANES == 2) {
+    int splits = sm_count() / tiles;  // one CTA per SM fits (shared memory): fill exactly one wave, no ragged tail
+    if (splits < min_chunks) splits = min_chunks;
+    if (splits > max_chunks) splits = max_chunks;
+    g.mblk_per_chunk = ceil_div(total_mblk, splits);
+    g.chunks = ceil_div(total_mblk, g.mblk_per_chunk);
+    grid = dim3(tiles, g.chunks);
+  } else {
+    long long best = -1;
+    for (int c = min_chunks; c <= max_chunks; ++c) {
+      const int per = ceil_div(total_mblk, c), chunks = ceil_div(total_mblk, per);
+      const long long span = (long long)ceil_div(tiles * chunks, sm_count()) * (per + 1);
+      if (best < 0 || span < best) {
+        best = span;
+        g.mblk_per_chunk = per;
+        g.chunks = chunks;
+      }
+    }
+    const int items = tiles * g.chunks;
+    grid = dim3(items < sm_count() ? items : sm_count());
+  }
+  DSVG_CUDA(launch_k(outer_kernel<BQ, NPLANES>, grid, dim3(Cfg::kThreads), Cfg::kSmemBytes, st, g,
+                     uint32_t(Cfg::kBoxBytes), 1024u));
   ++g_launches;
   return 0;
+}
+
+static void outer_problem(OuterGroup& g, int i, const float* alpha_dev, float alpha, float* C, int ldc, float* colsum,
+                          int P, int Q, int BQ) {
+  g.C[i] = C; g.colsum[i] = colsum; g.alpha_dev[i] = alpha_dev; g.alpha[i] = alpha;
+  g.P[i] = P; g.Q[i] = Q; g.ldc[i] = ldc;
+  g.vec[i] = int(ldc % 4 == 0 && Q % 4 == 0 && (reinterpret_cast<uintptr_t>(C) & 15) == 0);
+  g.tile_begin[i + 1] = g.tile_begin[i] + ceil_div(P, 128) * ceil_div(Q, BQ);
 }
 
 }  // namespace dsvg
@@ -1747,40 +1975,15 @@ extern "C" int dsvg_outer_group(int n, const dsvg_outer_problem* pr, int M, void
   OuterGroup g{};
   g.n = n;
   g.M = M;
-  int tiles_total = 0, tiles[kMaxGroup];
   for (int i = 0; i < n; ++i) {
     const dsvg_outer_problem& q = pr[i];
     DSVG_CHECK(q.A && q.B && q.C && q.P > 0 && q.Q > 0, "dsvg_outer_group: bad problem %d", i);
     DSVG_CHECK(q.lda % 8 == 0 && q.ldb % 8 == 0, "dsvg_outer_group: lda/ldb must be multiples of 8");
     if (make_map(&g.a[i], reinterpret_cast<const bf16*>(q.A), q.P, M, q.lda, 64, 64)) return 1;
     if (make_map(&g.b[i], reinterpret_cast<const bf16*>(q.B), q.Q, M, q.ldb, 64, 64)) return 1;
-    g.C[i] = q.C; g.colsum[i] = q.colsum_out; g.alpha_dev[i] = q.alpha_dev; g.alpha[i] = q.alpha;
-    g.P[i] = q.P; g.Q[i] = q.Q; g.ldc[i] = q.ldc;
-    g.vec[i] = int(q.ldc % 4 == 0 && q.Q % 4 == 0 && (reinterpret_cast<uintptr_t>(q.C) & 15) == 0);
-    tiles[i] = ceil_div(q.P, 128) * ceil_div(q.Q, 256);
-    tiles_total += tiles[i];
+    outer_problem(g, i, q.alpha_dev, q.alpha, q.C, q.ldc, q.colsum_out, q.P, q.Q, 256);
   }
-  const int total_mblk = ceil_div(M, 64);
-  int splits = sm_count() / tiles_total;
-  if (splits < ceil_div(total_mblk, kMaxSplitBlocks)) splits = ceil_div(total_mblk, kMaxSplitBlocks);
-  if (splits > total_mblk / 4) splits = total_mblk / 4;
-  if (splits < 1) splits = 1;
-  const int per = ceil_div(total_mblk, splits);
-  splits = ceil_div(total_mblk, per);
-  g.splits = splits;
-  g.mblk_per_split = per;
-  g.cta_begin[0] = 0;
-  for (int i = 0; i < n; ++i) g.cta_begin[i + 1] = g.cta_begin[i] + tiles[i] * splits;
-  for (int i = n; i < kMaxGroup; ++i) g.cta_begin[i + 1] = g.cta_begin[n];
-  using Cfg = OuterCfg<256, 1>;
-  static bool configured[kMaxDevices] = {};
-  if (first_use_on_device(configured)) {
-    DSVG_CUDA(cudaFuncSetAttribute(outer_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  }
-  DSVG_CUDA(launch_k(outer_group_kernel, dim3(g.cta_begin[n]), dim3(Cfg::kThreads), Cfg::kSmemBytes,
-                     static_cast<cudaStream_t>(stream), g, uint32_t(Cfg::kBoxBytes), 1024u));
-  ++g_launches;
-  return 0;
+  return launch_outer<256, 1>(g, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int dsvg_outer(const dsvg_bf16* A, size_t a_lo_off, int lda, const dsvg_bf16* B, size_t b_lo_off, int ldb,
@@ -1791,22 +1994,21 @@ extern "C" int dsvg_outer(const dsvg_bf16* A, size_t a_lo_off, int lda, const ds
   DSVG_CHECK(lda % 8 == 0 && ldb % 8 == 0, "dsvg_outer: lda/ldb must be multiples of 8");
   DSVG_CHECK((a_lo_off == 0) == (b_lo_off == 0), "dsvg_outer: both operands must have the same number of planes");
   const bool wide = (Q > 128);
-  CUtensorMap a, alo, b, blo;
+  OuterGroup g{};
+  g.n = 1;
+  g.M = M;
   const bf16* Ab = reinterpret_cast<const bf16*>(A);
   const bf16* Bb = reinterpret_cast<const bf16*>(B);
   // dim0 = feature columns (contiguous), dim1 = M rows; the tensor extents clip (zero-fill) ragged edges
-  if (make_map(&a, Ab, P, M, lda, 64, 64)) return 1;
-  if (make_map(&b, Bb, Q, M, ldb, 64, 64)) return 1;
-  alo = a;
-  blo = b;
+  if (make_map(&g.a[0], Ab, P, M, lda, 64, 64)) return 1;
+  if (make_map(&g.b[0], Bb, Q, M, ldb, 64, 64)) return 1;
   const bool split = a_lo_off != 0;
   if (split) {
-    if (make_map(&alo, Ab + a_lo_off, P, M, lda, 64, 64)) return 1;
-    if (make_map(&blo, Bb + b_lo_off, Q, M, ldb, 64, 64)) return 1;
+    if (make_map(&g.alo, Ab + a_lo_off, P, M, lda, 64, 64)) return 1;
+    if (make_map(&g.blo, Bb + b_lo_off, Q, M, ldb, 64, 64)) return 1;
   }
+  outer_problem(g, 0, alpha_dev, alpha, C, ldc, colsum_out, P, Q, wide ? 256 : 128);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (wide) return split ? launch_outer<256, 2>(a, alo, b, blo, M, P, Q, alpha, alpha_dev, C, ldc, colsum_out, st)
-                         : launch_outer<256, 1>(a, alo, b, blo, M, P, Q, alpha, alpha_dev, C, ldc, colsum_out, st);
-  return split ? launch_outer<128, 2>(a, alo, b, blo, M, P, Q, alpha, alpha_dev, C, ldc, colsum_out, st)
-               : launch_outer<128, 1>(a, alo, b, blo, M, P, Q, alpha, alpha_dev, C, ldc, colsum_out, st);
+  if (wide) return split ? launch_outer<256, 2>(g, st) : launch_outer<256, 1>(g, st);
+  return split ? launch_outer<128, 2>(g, st) : launch_outer<128, 1>(g, st);
 }
