@@ -1,7 +1,8 @@
 // Fast-mode attention for DeepSVG's tiny sequences on the warp-level tensor-core path (mma.sync m16n8k16, bf16 in,
-// fp32 accumulate): one warp owns one (sequence, head) pair, head_dim = 32, L <= 32 keys/queries padded to a
-// 32 x 32 tile.  Q, K, V (and dO in the backward) are staged in shared memory with coalesced 16-byte loads and
-// read back with ldmatrix; scores, probabilities and all gradients of the pair stay in registers / shared memory.
+// fp32 accumulate): one warp computes one (sequence, head) pair at a time, head_dim = 32, L <= 32 keys/queries padded
+// to a 32 x 32 tile.  Whole sequences stream through shared memory (bulk copies into a ring of stages, see "sequence
+// streaming" below) and are read with ldmatrix; scores, probabilities and all gradients of the pair stay in registers /
+// shared memory, and the outputs leave through shared memory as whole-row bulk stores.
 //
 //   reference: functional.py:168-248 (attention.cu keeps the fp32 SIMT version for head_dim 16 / L > 80; the parity-mode
 //   variants of these kernels -- two bf16 planes, three products -- follow further down in this file).  wgmma is not used here on purpose: a 32 x 32 x 32 problem fills a fraction of
@@ -11,6 +12,7 @@
 // identical in forward and backward of THIS kernel.
 #include "../../include/dsvg_b200.h"
 #include "common.cuh"
+#include "ptx.cuh"
 
 namespace dsvg {
 extern unsigned long long g_launches;
@@ -28,6 +30,7 @@ struct MmaAttnArgs {
   float scale;
   Dropout drop;
   int causal;           // query i sees keys j <= i only
+  int stages;           // attn_mma_fwd / bwd: shared-memory stages of the sequence ring (1 or 2)
 };
 
 __device__ __forceinline__ void mma_bf16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -52,26 +55,26 @@ __device__ __forceinline__ uint32_t smem_addr(const void* p) { return uint32_t(_
 
 // ---- fragment loaders (tile = 32 x 32 bf16, row stride kRow) -------------------------------------------
 // A operand, rows [16*mt, +16), k columns [16*ks, +16): a0..a3 from one ldmatrix.x4
-__device__ __forceinline__ void load_a(uint32_t (&a)[4], uint32_t tile, int mt, int ks, int lane) {
+__device__ __forceinline__ void load_a(uint32_t (&a)[4], uint32_t tile, int mt, int ks, int lane, int st = kRow) {
   const int m = lane >> 3, r = lane & 7;
-  ldsm_x4(a, tile + ((16 * mt + (m & 1) * 8 + r) * kRow + 16 * ks + (m >> 1) * 8) * 2);
+  ldsm_x4(a, tile + ((16 * mt + (m & 1) * 8 + r) * st + 16 * ks + (m >> 1) * 8) * 2);
 }
 // A operand taken TRANSPOSED from a row-major tile Z[k][m]: A[m][k] = Z[k][m]
-__device__ __forceinline__ void load_a_t(uint32_t (&a)[4], uint32_t tile, int mt, int ks, int lane) {
+__device__ __forceinline__ void load_a_t(uint32_t (&a)[4], uint32_t tile, int mt, int ks, int lane, int st = kRow) {
   const int m = lane >> 3, r = lane & 7;
   // matrices: (k0, m0) (k0, m0+8) (k0+8, m0) (k0+8, m0+8) -> a0 a1 a2 a3
-  ldsm_x4_t(a, tile + ((16 * ks + (m >> 1) * 8 + r) * kRow + 16 * mt + (m & 1) * 8) * 2);
+  ldsm_x4_t(a, tile + ((16 * ks + (m >> 1) * 8 + r) * st + 16 * mt + (m & 1) * 8) * 2);
 }
 // B operand ("col") for two adjacent n-tiles from row-major X[n][k] (K for Q.K^T, V for dO.V^T):
 // r0,r1 = b0,b1 of n-tile 2*np ; r2,r3 = b0,b1 of n-tile 2*np+1
-__device__ __forceinline__ void load_b_nk(uint32_t (&b)[4], uint32_t tile, int np, int ks, int lane) {
+__device__ __forceinline__ void load_b_nk(uint32_t (&b)[4], uint32_t tile, int np, int ks, int lane, int st = kRow) {
   const int m = lane >> 3, r = lane & 7;
-  ldsm_x4(b, tile + ((16 * np + (m >> 1) * 8 + r) * kRow + 16 * ks + (m & 1) * 8) * 2);
+  ldsm_x4(b, tile + ((16 * np + (m >> 1) * 8 + r) * st + 16 * ks + (m & 1) * 8) * 2);
 }
 // B operand for two adjacent n-tiles from row-major Y[k][n] (V for P.V, K for dS.K, Q / dO for the transposed products)
-__device__ __forceinline__ void load_b_kn(uint32_t (&b)[4], uint32_t tile, int np, int ks, int lane) {
+__device__ __forceinline__ void load_b_kn(uint32_t (&b)[4], uint32_t tile, int np, int ks, int lane, int st = kRow) {
   const int m = lane >> 3, r = lane & 7;
-  ldsm_x4_t(b, tile + ((16 * ks + (m & 1) * 8 + r) * kRow + 16 * np + (m >> 1) * 8) * 2);
+  ldsm_x4_t(b, tile + ((16 * ks + (m & 1) * 8 + r) * st + 16 * np + (m >> 1) * 8) * 2);
 }
 
 // stage a [L x 32] head slice (row stride ld elements) into a zero-padded 32 x 32 tile; 16-byte chunks
@@ -155,8 +158,9 @@ __device__ __forceinline__ uint32_t key_mask_of(const uint8_t* valid, size_t row
   return __ballot_sync(0xffffffffu, ok);
 }
 
-// S = Q K^T  (both tiles row-major [row][channel])
-__device__ __forceinline__ void qk_scores(float (&s)[2][4][4], uint32_t q_tile, uint32_t k_tile, int lane) {
+// S = Q K^T  (both tiles row-major [row][channel]; qs, kst: their row strides in elements)
+__device__ __forceinline__ void qk_scores(float (&s)[2][4][4], uint32_t q_tile, uint32_t k_tile, int lane, int qs = kRow,
+                                          int kst = kRow) {
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
@@ -166,12 +170,12 @@ __device__ __forceinline__ void qk_scores(float (&s)[2][4][4], uint32_t q_tile, 
 #pragma unroll
   for (int ks = 0; ks < 2; ++ks) {
     uint32_t a[2][4];
-    load_a(a[0], q_tile, 0, ks, lane);
-    load_a(a[1], q_tile, 1, ks, lane);
+    load_a(a[0], q_tile, 0, ks, lane, qs);
+    load_a(a[1], q_tile, 1, ks, lane, qs);
 #pragma unroll
     for (int np = 0; np < 2; ++np) {
       uint32_t b[4];
-      load_b_nk(b, k_tile, np, ks, lane);
+      load_b_nk(b, k_tile, np, ks, lane, kst);
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt) {
         mma_bf16(s[mt][2 * np], a[mt], b[0], b[1]);
@@ -188,8 +192,9 @@ __device__ __forceinline__ void c_to_a(uint32_t (&a)[4], const float (&c)[2][4][
   a[2] = pack_bf16(c[mt][2 * ks + 1][0], c[mt][2 * ks + 1][1]);
   a[3] = pack_bf16(c[mt][2 * ks + 1][2], c[mt][2 * ks + 1][3]);
 }
-// out[32 x 32] = A(regs, from c_to_a) . Y   with Y row-major [k][n] in smem
-__device__ __forceinline__ void mul_regs_kn(float (&o)[2][4][4], const float (&p)[2][4][4], uint32_t y_tile, int lane) {
+// out[32 x 32] = A(regs, from c_to_a) . Y   with Y row-major [k][n] in smem (row stride ys elements)
+__device__ __forceinline__ void mul_regs_kn(float (&o)[2][4][4], const float (&p)[2][4][4], uint32_t y_tile, int lane,
+                                            int ys = kRow) {
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
@@ -204,7 +209,7 @@ __device__ __forceinline__ void mul_regs_kn(float (&o)[2][4][4], const float (&p
 #pragma unroll
     for (int np = 0; np < 2; ++np) {
       uint32_t b[4];
-      load_b_kn(b, y_tile, np, ks, lane);
+      load_b_kn(b, y_tile, np, ks, lane, ys);
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt) {
         mma_bf16(o[mt][2 * np], a[mt], b[0], b[1]);
@@ -213,8 +218,9 @@ __device__ __forceinline__ void mul_regs_kn(float (&o)[2][4][4], const float (&p
     }
   }
 }
-// out[32 x 32] = Z^T . Y   with Z, Y row-major [k][.] in smem (contraction over the smem row index)
-__device__ __forceinline__ void mul_t_kn(float (&o)[2][4][4], uint32_t z_tile, uint32_t y_tile, int lane) {
+// out[32 x 32] = Z^T . Y   with Z, Y row-major [k][.] in smem (contraction over the smem row index; row strides zs, ys)
+__device__ __forceinline__ void mul_t_kn(float (&o)[2][4][4], uint32_t z_tile, uint32_t y_tile, int lane, int zs = kRow,
+                                         int ys = kRow) {
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
@@ -224,12 +230,12 @@ __device__ __forceinline__ void mul_t_kn(float (&o)[2][4][4], uint32_t z_tile, u
 #pragma unroll
   for (int ks = 0; ks < 2; ++ks) {
     uint32_t a[2][4];
-    load_a_t(a[0], z_tile, 0, ks, lane);
-    load_a_t(a[1], z_tile, 1, ks, lane);
+    load_a_t(a[0], z_tile, 0, ks, lane, zs);
+    load_a_t(a[1], z_tile, 1, ks, lane, zs);
 #pragma unroll
     for (int np = 0; np < 2; ++np) {
       uint32_t b[4];
-      load_b_kn(b, y_tile, np, ks, lane);
+      load_b_kn(b, y_tile, np, ks, lane, ys);
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt) {
         mma_bf16(o[mt][2 * np], a[mt], b[0], b[1]);
@@ -238,9 +244,9 @@ __device__ __forceinline__ void mul_t_kn(float (&o)[2][4][4], uint32_t z_tile, u
     }
   }
 }
-// store a C-fragment as bf16 to global rows [row0 + i] (i < L), 32 channels starting at dst
-__device__ __forceinline__ void store_c_global(bf16* dst, int ld, int L, const float (&c)[2][4][4], float mul, int g,
-                                               int t) {
+// store a C-fragment as bf16 (times mul) to rows i < L of a row-major smem tile with row stride st elements; rows >= L
+// are left as they are (the zero padding of the streamed tiles)
+__device__ __forceinline__ void store_c_rows(bf16* tile, int st, int L, const float (&c)[2][4][4], float mul, int g, int t) {
 #pragma unroll
   for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
@@ -249,7 +255,7 @@ __device__ __forceinline__ void store_c_global(bf16* dst, int ld, int L, const f
       if (i < L) {
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt)
-          *reinterpret_cast<uint32_t*>(dst + size_t(i) * ld + 8 * nt + 2 * t) =
+          *reinterpret_cast<uint32_t*>(tile + i * st + 8 * nt + 2 * t) =
               pack_bf16(c[mt][nt][2 * hrow] * mul, c[mt][nt][2 * hrow + 1] * mul);
       }
     }
@@ -266,127 +272,224 @@ __device__ __forceinline__ void store_c_smem(bf16* tile, const float (&c)[2][4][
     }
 }
 
-constexpr int kMmaWarps = 4;
+// ---- sequence streaming ------------------------------------------------------------------------------------------
+// The rows of a sequence are contiguous in qkv [nseq*L, 3d] (and dout [nseq*L, d]), so the kernels move whole sequences:
+// CTAs are persistent (one wave) and walk the sequences blockIdx.x, + gridDim.x, ...  A producer warp (the last warp)
+// copies each sequence into a ring of `stages` shared-memory stages with one bulk copy per row (lane r: row r), completed
+// on the stage's `full` mbarrier, while the consumer warps compute the sequence before it.  Consumer warp w takes heads
+// w, w + W, ... of the sequence (W = min(H, kStreamWarps)); every (sequence, head) pair runs exactly the arithmetic of the
+// earlier warp-per-pair kernels, and its dropout pair index stays seq * H + h.
+//
+// A stage holds 32 qkv rows with a stride of 3d + 8 elements (and, in the backward, 32 dO rows with a stride of d + 8):
+// 16 * odd bytes, so ldmatrix on a head's 32-column slice is free of bank conflicts.  Rows >= L are zeroed once when the
+// kernel starts and never written again -- no copy covers them and every output store skips them -- so the padded rows
+// of the 32 x 32 tiles reach the MMAs as zeros, as the backward requires (zero Q / dO rows make dS and the dV
+// contributions of padded query rows exactly 0).  Outputs are written in place into the stage (o over the head's Q
+// columns; dq, dk, dv over Q, K, V) and leave as one bulk store per row, issued by the producer once every consumer has
+// released the stage; the producer waits until those stores have read the stage before it refills it.
+constexpr int kStreamWarps = 8;          // consumer warps per CTA at most
+constexpr int kStreamRows = 32;          // rows of a stage (the 32 x 32 tile height)
+constexpr int kStreamMaxStages = 2;
+constexpr int kStreamBarBytes = 64;      // full[kStreamMaxStages], empty[kStreamMaxStages] ahead of the stages
+constexpr int kStreamSmemMax = 227 * 1024;
 
-__global__ void __launch_bounds__(kMmaWarps * 32) attn_mma_fwd_kernel(MmaAttnArgs a) {
-  pdl_launch_dependents();
-  pdl_wait();
-  drop_resolve(a.drop);
-  __shared__ __align__(16) bf16 sm[kMmaWarps][3 * kTile];
-  const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const int L = a.L, d = a.H * 32, ld = 3 * d;
-  bf16* Qs = sm[wib];
-  bf16* Ks = Qs + kTile;
-  bf16* Vs = Ks + kTile;
-  const uint32_t q_t = smem_addr(Qs), k_t = smem_addr(Ks), v_t = smem_addr(Vs);
-  const long long npairs = (long long)a.nseq * a.H;
-  for (long long pair = (long long)blockIdx.x * kMmaWarps + wib; pair < npairs; pair += (long long)gridDim.x * kMmaWarps) {
-    const int seq = int(pair / a.H), h = int(pair % a.H);
-    const size_t row0 = size_t(seq) * L;
-    const bf16* base = a.qkv + row0 * ld + h * 32;
-    stage_tile(Qs, base, ld, L, lane);
-    stage_tile(Ks, base + d, ld, L, lane);
-    stage_tile(Vs, base + 2 * d, ld, L, lane);
-    const uint32_t kmask = key_mask_of(a.valid, row0, L, lane);
-    __syncwarp();
-    float s[2][4][4];
-    qk_scores(s, q_t, k_t, lane);
-    softmax_rows(s, kmask, t, g, a.causal);
-    if (a.drop.p > 0.f) {
-      float mult[2][4][4];
-      dropout_tile(mult, a.drop, (unsigned long long)pair, g, t);
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) s[mt][nt][e] *= mult[mt][nt][e];
-    }
-    float o[2][4][4];
-    mul_regs_kn(o, s, v_t, lane);
-    store_c_global(a.out + row0 * d + h * 32, d, L, o, 1.f, g, t);
-    __syncwarp();
-  }
+__host__ __device__ constexpr int stream_qkv_stride(int H) { return 96 * H + 8; }
+__host__ __device__ constexpr int stream_dout_stride(int H) { return 32 * H + 8; }
+// elements of one stage
+__host__ __device__ constexpr int stream_stage_elems(int H, bool bwd) {
+  return kStreamRows * (stream_qkv_stride(H) + (bwd ? stream_dout_stride(H) : 0));
 }
 
-__global__ void __launch_bounds__(kMmaWarps * 32) attn_mma_bwd_kernel(MmaAttnArgs a) {
-  pdl_launch_dependents();
-  pdl_wait();
-  drop_resolve(a.drop);
-  extern __shared__ __align__(16) bf16 sm_dyn[];   // kMmaWarps x 6 tiles (60 KB: above the static limit)
-  const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const int L = a.L, d = a.H * 32, ld = 3 * d;
-  bf16* Qs = sm_dyn + wib * 6 * kTile;
-  bf16* Ks = Qs + kTile;
-  bf16* Vs = Ks + kTile;
-  bf16* Gs = Vs + kTile;   // dO
-  bf16* Ps = Gs + kTile;   // dropout-scaled probabilities
-  bf16* Ds = Ps + kTile;   // dS
-  const uint32_t q_t = smem_addr(Qs), k_t = smem_addr(Ks), v_t = smem_addr(Vs), g_t = smem_addr(Gs),
-                 p_t = smem_addr(Ps), d_t = smem_addr(Ds);
-  const long long npairs = (long long)a.nseq * a.H;
-  for (long long pair = (long long)blockIdx.x * kMmaWarps + wib; pair < npairs; pair += (long long)gridDim.x * kMmaWarps) {
-    const int seq = int(pair / a.H), h = int(pair % a.H);
-    const size_t row0 = size_t(seq) * L;
-    const bf16* base = a.qkv + row0 * ld + h * 32;
-    stage_tile(Qs, base, ld, L, lane);
-    stage_tile(Ks, base + d, ld, L, lane);
-    stage_tile(Vs, base + 2 * d, ld, L, lane);
-    stage_tile(Gs, a.dout + row0 * d + h * 32, d, L, lane);
-    const uint32_t kmask = key_mask_of(a.valid, row0, L, lane);
-    __syncwarp();
-    float p[2][4][4], dp[2][4][4];
-    qk_scores(p, q_t, k_t, lane);
-    softmax_rows(p, kmask, t, g, a.causal);
-    qk_scores(dp, g_t, v_t, lane);            // dP = dO . V^T  (same operand shapes as Q . K^T)
-    if (a.drop.p > 0.f) {
-      float mult[2][4][4];
-      dropout_tile(mult, a.drop, (unsigned long long)pair, g, t);
-#pragma unroll
-      for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            dp[mt][nt][e] *= mult[mt][nt][e];   // d loss / d p  (through the dropout)
-            mult[mt][nt][e] *= p[mt][nt][e];    // dropout-scaled probability (operand of dV)
-          }
-      store_c_smem(Ps, mult, g, t);
-    } else {
-      store_c_smem(Ps, p, g, t);
+// zero every stage, initialise the barriers; all threads, before any copy is issued
+__device__ __forceinline__ void stream_init(unsigned char* smem, int stage_bytes, int stages, int consumers) {
+  uint4* z = reinterpret_cast<uint4*>(smem + kStreamBarBytes);
+  for (int i = threadIdx.x; i < stages * stage_bytes / 16; i += blockDim.x) z[i] = make_uint4(0, 0, 0, 0);
+  fence_proxy_async_smem();   // the zeros precede the bulk copies (async proxy) into the same stage
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < stages; ++s) {
+      mbar_init(&bars[s], 1);
+      mbar_init(&bars[kStreamMaxStages + s], consumers);
     }
-    // dS = P o (dP - rowsum(dP o P))
-#pragma unroll
-    for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-      for (int hrow = 0; hrow < 2; ++hrow) {
-        float delta = 0.f;
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) delta = fmaf(dp[mt][nt][2 * hrow + e], p[mt][nt][2 * hrow + e], delta);
-        delta += __shfl_xor_sync(0xffffffffu, delta, 1);
-        delta += __shfl_xor_sync(0xffffffffu, delta, 2);
-#pragma unroll
-        for (int nt = 0; nt < 4; ++nt)
-#pragma unroll
-          for (int e = 0; e < 2; ++e)
-            dp[mt][nt][2 * hrow + e] = p[mt][nt][2 * hrow + e] * (dp[mt][nt][2 * hrow + e] - delta);
+    fence_barrier_init();
+  }
+  __syncthreads();
+}
+
+// Producer warp: iteration k loads the CTA's k-th sequence into stage k % stages; first it stores the outputs of
+// sequence k - stages out of that stage (once all consumers released it) and waits until the stores have read it.
+// qkv rows (and dout rows) in; out_cols leading columns of each stage row out, to rows of `dst` with stride dst_ld.
+__device__ __forceinline__ void stream_producer(unsigned char* smem, int stage_elems, int stages, const MmaAttnArgs& a,
+                                                bool bwd, int lane) {
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem);
+  uint64_t* empty = full + kStreamMaxStages;
+  bf16* stage0 = reinterpret_cast<bf16*>(smem + kStreamBarBytes);
+  const int L = a.L, d = a.H * 32, rs = stream_qkv_stride(a.H), rd = stream_dout_stride(a.H);
+  const int n = (a.nseq - int(blockIdx.x) + int(gridDim.x) - 1) / int(gridDim.x);
+  const uint32_t row_in = uint32_t(3 * d * 2 + (bwd ? d * 2 : 0));
+  const int out_cols = bwd ? 3 * d : d;
+  bf16* dst = bwd ? a.dqkv : a.out;
+  for (int k = 0; k < n + stages; ++k) {
+    const int s = k % stages;
+    bf16* qkv_st = stage0 + size_t(s) * stage_elems;
+    if (k >= stages) {
+      mbar_wait(&empty[s], uint32_t((k / stages - 1) & 1));
+      const size_t row0 = size_t(int(blockIdx.x) + (k - stages) * int(gridDim.x)) * L;
+      if (lane < L) bulk_store(dst + (row0 + lane) * out_cols, qkv_st + lane * rs, uint32_t(out_cols * 2));
+      tma_store_commit();
+    }
+    if (k < n) {
+      if (k >= stages) tma_store_wait_read();   // this lane's row of the stage has been read out
+      const size_t row0 = size_t(int(blockIdx.x) + k * int(gridDim.x)) * L;
+      if (lane == 0) mbar_arrive_expect_tx(&full[s], uint32_t(L) * row_in);
+      __syncwarp();
+      if (lane < L) {
+        bulk_load(qkv_st + lane * rs, a.qkv + (row0 + lane) * (3 * d), uint32_t(3 * d * 2), &full[s]);
+        if (bwd)
+          bulk_load(qkv_st + kStreamRows * rs + lane * rd, a.dout + (row0 + lane) * d, uint32_t(d * 2), &full[s]);
       }
-    store_c_smem(Ds, dp, g, t);
-    __syncwarp();
-    float o[2][4][4];
-    bf16* dbase = a.dqkv + row0 * ld + h * 32;
-    mul_regs_kn(o, dp, k_t, lane);                 // dQ = dS . K
-    store_c_global(dbase, ld, L, o, a.scale, g, t);
-    mul_t_kn(o, d_t, q_t, lane);                   // dK = dS^T . Q
-    store_c_global(dbase + d, ld, L, o, 1.f, g, t);
-    mul_t_kn(o, p_t, g_t, lane);                   // dV = (dropout(P))^T . dO
-    store_c_global(dbase + 2 * d, ld, L, o, 1.f, g, t);
-    __syncwarp();
+    }
+  }
+  tma_store_wait_all();   // the stores have completed before the CTA exits
+}
+
+__global__ void __launch_bounds__((kStreamWarps + 1) * 32, 2) attn_mma_fwd_kernel(MmaAttnArgs a) {
+  pdl_launch_dependents();
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int W = int(blockDim.x >> 5) - 1, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int L = a.L, H = a.H, d = H * 32, rs = stream_qkv_stride(H), stages = a.stages;
+  const int stage_elems = stream_stage_elems(H, false);
+  stream_init(smem, stage_elems * 2, stages, W * 32);
+  pdl_wait();
+  if (warp == W) {
+    stream_producer(smem, stage_elems, stages, a, false, lane);
+    return;
+  }
+  drop_resolve(a.drop);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem);
+  uint64_t* empty = full + kStreamMaxStages;
+  bf16* stage0 = reinterpret_cast<bf16*>(smem + kStreamBarBytes);
+  const int n = (a.nseq - int(blockIdx.x) + int(gridDim.x) - 1) / int(gridDim.x);
+  for (int k = 0; k < n; ++k) {
+    const int s = k % stages, seq = int(blockIdx.x) + k * int(gridDim.x);
+    const size_t row0 = size_t(seq) * L;
+    const uint32_t kmask = key_mask_of(a.valid, row0, L, lane);
+    bf16* st = stage0 + size_t(s) * stage_elems;
+    mbar_wait(&full[s], uint32_t((k / stages) & 1));
+    for (int h = warp; h < H; h += W) {
+      bf16* Qs = st + h * 32;
+      const uint32_t q_t = smem_addr(Qs), k_t = smem_addr(Qs + d), v_t = smem_addr(Qs + 2 * d);
+      const long long pair = (long long)seq * H + h;
+      float sc[2][4][4];
+      qk_scores(sc, q_t, k_t, lane, rs, rs);
+      softmax_rows(sc, kmask, t, g, a.causal);
+      if (a.drop.p > 0.f) {
+        float mult[2][4][4];
+        dropout_tile(mult, a.drop, (unsigned long long)pair, g, t);
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) sc[mt][nt][e] *= mult[mt][nt][e];
+      }
+      float o[2][4][4];
+      mul_regs_kn(o, sc, v_t, lane, rs);
+      __syncwarp();                                // every lane is done with this head's Q
+      store_c_rows(Qs, rs, L, o, 1.f, g, t);       // o over Q: the producer stores the first d columns of each row
+    }
+    fence_proxy_async_smem();                      // the generic-proxy writes above precede the bulk store that reads them
+    mbar_arrive(&empty[s]);
   }
 }
 
+__global__ void __launch_bounds__((kStreamWarps + 1) * 32, 1) attn_mma_bwd_kernel(MmaAttnArgs a) {
+  pdl_launch_dependents();
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int W = int(blockDim.x >> 5) - 1, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+  const int L = a.L, H = a.H, d = H * 32, rs = stream_qkv_stride(H), rd = stream_dout_stride(H), stages = a.stages;
+  const int stage_elems = stream_stage_elems(H, true);
+  stream_init(smem, stage_elems * 2, stages, W * 32);
+  pdl_wait();
+  if (warp == W) {
+    stream_producer(smem, stage_elems, stages, a, true, lane);
+    return;
+  }
+  drop_resolve(a.drop);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem);
+  uint64_t* empty = full + kStreamMaxStages;
+  bf16* stage0 = reinterpret_cast<bf16*>(smem + kStreamBarBytes);
+  bf16* Ps = stage0 + size_t(stages) * stage_elems + warp * 2 * kTile;   // dropout-scaled probabilities (per warp)
+  bf16* Ds = Ps + kTile;                                                 // dS
+  const uint32_t p_t = smem_addr(Ps), d_t = smem_addr(Ds);
+  const int n = (a.nseq - int(blockIdx.x) + int(gridDim.x) - 1) / int(gridDim.x);
+  for (int k = 0; k < n; ++k) {
+    const int s = k % stages, seq = int(blockIdx.x) + k * int(gridDim.x);
+    const size_t row0 = size_t(seq) * L;
+    const uint32_t kmask = key_mask_of(a.valid, row0, L, lane);
+    bf16* st = stage0 + size_t(s) * stage_elems;
+    mbar_wait(&full[s], uint32_t((k / stages) & 1));
+    for (int h = warp; h < H; h += W) {
+      bf16* Qs = st + h * 32;
+      bf16* Ks = Qs + d;
+      bf16* Vs = Qs + 2 * d;
+      bf16* Gs = st + kStreamRows * rs + h * 32;   // dO
+      const uint32_t q_t = smem_addr(Qs), k_t = smem_addr(Ks), v_t = smem_addr(Vs), g_t = smem_addr(Gs);
+      const long long pair = (long long)seq * H + h;
+      float p[2][4][4], dp[2][4][4];
+      qk_scores(p, q_t, k_t, lane, rs, rs);
+      softmax_rows(p, kmask, t, g, a.causal);
+      qk_scores(dp, g_t, v_t, lane, rd, rs);       // dP = dO . V^T  (same operand shapes as Q . K^T)
+      if (a.drop.p > 0.f) {
+        float mult[2][4][4];
+        dropout_tile(mult, a.drop, (unsigned long long)pair, g, t);
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              dp[mt][nt][e] *= mult[mt][nt][e];   // d loss / d p  (through the dropout)
+              mult[mt][nt][e] *= p[mt][nt][e];    // dropout-scaled probability (operand of dV)
+            }
+        store_c_smem(Ps, mult, g, t);
+      } else {
+        store_c_smem(Ps, p, g, t);
+      }
+      // dS = P o (dP - rowsum(dP o P))
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int hrow = 0; hrow < 2; ++hrow) {
+          float delta = 0.f;
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) delta = fmaf(dp[mt][nt][2 * hrow + e], p[mt][nt][2 * hrow + e], delta);
+          delta += __shfl_xor_sync(0xffffffffu, delta, 1);
+          delta += __shfl_xor_sync(0xffffffffu, delta, 2);
+#pragma unroll
+          for (int nt = 0; nt < 4; ++nt)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              dp[mt][nt][2 * hrow + e] = p[mt][nt][2 * hrow + e] * (dp[mt][nt][2 * hrow + e] - delta);
+        }
+      store_c_smem(Ds, dp, g, t);
+      __syncwarp();
+      float oq[2][4][4], ok[2][4][4];
+      mul_regs_kn(oq, dp, k_t, lane, rs);          // dQ = dS . K
+      mul_t_kn(ok, d_t, q_t, lane, kRow, rs);      // dK = dS^T . Q
+      __syncwarp();                                // every lane is done with this head's Q and K (V: since dP)
+      store_c_rows(Qs, rs, L, oq, a.scale, g, t);
+      store_c_rows(Ks, rs, L, ok, 1.f, g, t);
+      mul_t_kn(oq, p_t, g_t, lane, kRow, rd);      // dV = (dropout(P))^T . dO
+      store_c_rows(Vs, rs, L, oq, 1.f, g, t);
+      __syncwarp();                                // Ps / Ds are rewritten for the next head
+    }
+    fence_proxy_async_smem();                      // the generic-proxy writes above precede the bulk store that reads them
+    mbar_arrive(&empty[s]);
+  }
+}
 
 // ================================================================================================================
 // Parity mode ("bf16x3") on the same 32 x 32 tiles: every activation is a (hi, lo) pair of bf16 planes carrying ~16
@@ -672,17 +775,34 @@ __global__ void __launch_bounds__(kX3Warps * 32) attn_x3_bwd_kernel(X3AttnArgs x
 }  // namespace dsvg
 using namespace dsvg;
 
-// Grid of the 32 x 32 kernels: exactly one wave of resident CTAs (the kernels stride over the pairs); measured against the
-// round-1 cap of 32 CTAs per SM: forward equal (75.2 vs 75.6 us), backward 137.7 vs 142.7 us at (4096 x 32, head_dim 32).
-static long long mma_grid_cap(bool bwd) {
-  static long long cap[2] = {0, 0};
-  if (cap[bwd] == 0) {
-    int n = 0;
-    if (bwd) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, dsvg::attn_mma_bwd_kernel, dsvg::kMmaWarps * 32, size_t(dsvg::kMmaWarps * 6 * dsvg::kTile * 2));
-    else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, dsvg::attn_mma_fwd_kernel, dsvg::kMmaWarps * 32, 0);
-    cap[bwd] = 132LL * (n > 0 ? n : 8);
-  }
-  return cap[bwd];
+// Launch of the sequence-streaming 32 x 32 kernels: W = min(H, kStreamWarps) consumer warps plus the producer warp, two
+// stages when they fit in shared memory (one otherwise), and exactly one wave of resident CTAs (at most one per sequence).
+static int launch_stream(bool bwd, MmaAttnArgs& a, cudaStream_t st) {
+  DSVG_CHECK(a.L >= 1 && a.L <= kStreamRows, "attn_mma: L = %d outside 1..%d", a.L, kStreamRows);
+  const uintptr_t align = reinterpret_cast<uintptr_t>(a.qkv) | reinterpret_cast<uintptr_t>(a.out) |
+                          reinterpret_cast<uintptr_t>(a.dout) | reinterpret_cast<uintptr_t>(a.dqkv);   // unused ones are null
+  DSVG_CHECK((align & 15) == 0, "attn_mma: qkv / dout / outputs must be 16-byte aligned for the bulk copies");
+  const int W = a.H < kStreamWarps ? a.H : kStreamWarps;
+  const long long stage = 2LL * stream_stage_elems(a.H, bwd);
+  const long long fixed = kStreamBarBytes + (bwd ? 2LL * W * 2 * kTile : 0);   // + per-warp P / dS tiles
+  a.stages = fixed + 2 * stage <= kStreamSmemMax ? 2 : 1;
+  const long long smem = fixed + a.stages * stage;
+  DSVG_CHECK(smem <= kStreamSmemMax, "attn_mma: H = %d heads need %lld bytes of shared memory per sequence (max %d)", a.H,
+             smem, kStreamSmemMax);
+  auto kern = bwd ? attn_mma_bwd_kernel : attn_mma_fwd_kernel;
+  static bool configured[2][kMaxDevices] = {};
+  if (first_use_on_device(configured[bwd]))
+    DSVG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kStreamSmemMax));
+  int dev = 0, sms = 0, per_sm = 0;
+  DSVG_CUDA(cudaGetDevice(&dev));
+  DSVG_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  DSVG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, (W + 1) * 32, size_t(smem)));
+  DSVG_CHECK(per_sm > 0, "attn_mma: %lld bytes of shared memory per CTA do not fit", smem);
+  long long blocks = (long long)sms * per_sm;
+  if (blocks > a.nseq) blocks = a.nseq;
+  DSVG_CUDA(launch_k(kern, dim3(int(blocks)), dim3((W + 1) * 32), size_t(smem), st, a));
+  ++g_launches;
+  return 0;
 }
 
 // Entry points used by attention.cu's dispatcher (not part of the public header: same ABI functions, faster path).
@@ -691,27 +811,14 @@ int dsvg_attn_mma_fwd(const bf16* qkv, const uint8_t* valid, bf16* out, int nseq
   MmaAttnArgs a{};
   a.qkv = qkv; a.valid = valid; a.out = out; a.nseq = nseq; a.L = L; a.H = H; a.scale = 1.f; a.drop = drop;
   a.causal = causal;
-  long long blocks = ((long long)nseq * H + kMmaWarps - 1) / kMmaWarps;
-  if (blocks > mma_grid_cap(false)) blocks = mma_grid_cap(false);
-  DSVG_CUDA(launch_k(attn_mma_fwd_kernel, dim3(int(blocks)), dim3(kMmaWarps * 32), 0, st, a));
-  ++g_launches;
-  return 0;
+  return launch_stream(false, a, st);
 }
 int dsvg_attn_mma_bwd(const bf16* qkv, const uint8_t* valid, const bf16* dout, bf16* dqkv, int nseq, int L, int H,
                       float q_scale, Dropout drop, int causal, cudaStream_t st) {
   MmaAttnArgs a{};
   a.qkv = qkv; a.valid = valid; a.dout = dout; a.dqkv = dqkv; a.nseq = nseq; a.L = L; a.H = H; a.scale = q_scale;
   a.drop = drop; a.causal = causal;
-  constexpr int smem = kMmaWarps * 6 * kTile * 2;
-  static bool configured[kMaxDevices] = {};
-  if (first_use_on_device(configured)) {
-    DSVG_CUDA(cudaFuncSetAttribute(attn_mma_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  }
-  long long blocks = ((long long)nseq * H + kMmaWarps - 1) / kMmaWarps;
-  if (blocks > mma_grid_cap(true)) blocks = mma_grid_cap(true);
-  DSVG_CUDA(launch_k(attn_mma_bwd_kernel, dim3(int(blocks)), dim3(kMmaWarps * 32), size_t(smem), st, a));
-  ++g_launches;
-  return 0;
+  return launch_stream(true, a, st);
 }
 
 // Parity-mode (two-plane) entry point of the 32 x 32 kernels.

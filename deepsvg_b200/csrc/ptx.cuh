@@ -86,6 +86,18 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* s
                "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
                : "memory");
 }
+// 1-D bulk copies (contiguous bytes, 16-byte aligned, size a multiple of 16): global -> shared completed on an mbarrier,
+// shared -> global in the bulk async group of the issuing thread (tma_store_commit / tma_store_wait_* apply).
+__device__ __forceinline__ void bulk_load(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+__device__ __forceinline__ void bulk_store(void* dst, const void* smem_src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
+               ::"l"(reinterpret_cast<uint64_t>(dst)), "r"(smem_u32(smem_src)), "r"(bytes)
+               : "memory");
+}
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // all committed bulk stores have finished READING shared memory (the buffer may be overwritten)
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
